@@ -90,9 +90,10 @@ class Grid:
         return out
 
 
-def fuse_vector(grid, pts, T_world_frame, Pl, W, H, radius):
+def fuse_vector(grid, pts, T_world_frame, Pl, W, H, radius, stats=None):
     """DepthFusion::update (:71-87) of one vector of points (dicts: p_cam, s2, nu, res, age, T_world_cam) into `grid`, Tdist norm.
-    Returns the number of fusions."""
+    Returns the number of fusions; stats (dict, optional) counts the branches taken: create, fuse, occluded, replace, keep."""
+    count = (lambda k: stats.__setitem__(k, stats.get(k, 0) + 1)) if stats is not None else (lambda k: None)
     T_frame_world = np.linalg.inv(np.asarray(T_world_frame, float).reshape(4, 4))
     n_fusion = 0
     for p in pts:
@@ -118,6 +119,7 @@ def fuse_vector(grid, pts, T_world_frame, Pl, W, H, radius):
                 nw.res, nw.age = prop.res, prop.age
                 nw.p_cam = ind.cam2world(Pl, nw.x, prop.rho)
                 grid.set(r, c, nw)
+                count("create")
                 continue
             cur = grid.cell[(r, c)]
             diff = abs(prop.rho - cur.rho)                                                                   # studentTCompatibleTest (:218-231)
@@ -127,11 +129,16 @@ def fuse_vector(grid, pts, T_world_frame, Pl, W, H, radius):
                 cur.res = min(cur.res, prop.res)
                 cur.p_cam = ind.cam2world(Pl, cur.x, prop.rho)
                 n_fusion += 1
+                count("fuse")
             else:                                                                                            # case 2.2 (:178-188)
                 if cur.rho - 2 * math.sqrt(cur.var) > prop.rho:
+                    count("occluded")
                     continue
                 if prop.var < cur.var and prop.res < cur.res:
                     grid.assign(r, c, prop)
+                    count("replace")
+                else:
+                    count("keep")
     return n_fusion
 
 
@@ -169,10 +176,12 @@ def regularize(grid, radius, min_nb, min_close, literal=True):
     return tmp
 
 
-def naive_propagate_vector(grid, pts, T_world_frame, Pl, W, H):
+def naive_propagate_vector(grid, pts, T_world_frame, Pl, W, H, stats=None):
     """DepthFusion::naive_propagation (DepthFusion.cpp:232-288) with naive_propagate_one_point (:290-327): Gaussian propagation,
     the four pixels around the re-projection, an empty pixel takes the point, an occupied one keeps the closer estimate and is
-    replaced only by a propagated point with a smaller residual.  pts: dicts p_cam, var, res, age, T_world_cam."""
+    replaced only by a propagated point with a smaller residual.  pts: dicts p_cam, var, res, age, T_world_cam.  stats (dict,
+    optional) counts the branches taken: create, nearer, replace, keep."""
+    count = (lambda k: stats.__setitem__(k, stats.get(k, 0) + 1)) if stats is not None else (lambda k: None)
     T_frame_world = np.linalg.inv(np.asarray(T_world_frame, float).reshape(4, 4))
     for p in pts:
         T = T_frame_world @ np.asarray(p["T_world_cam"], float).reshape(4, 4)
@@ -199,9 +208,14 @@ def naive_propagate_vector(grid, pts, T_world_frame, Pl, W, H):
                     nw.res, nw.age = prop.res, prop.age
                     nw.p_cam = ind.cam2world(Pl, nw.x, prop.rho)
                     grid.set(r, c, nw)
+                    count("create")
                 else:                                                       # case 2
                     cur = grid.cell[(r, c)]
                     if cur.rho > prop.rho:
+                        count("nearer")
                         continue
                     if prop.res < cur.res:
                         grid.assign(r, c, prop)
+                        count("replace")
+                    else:
+                        count("keep")

@@ -63,12 +63,21 @@ def patch_interpolation(img, loc, wx, wy):
     return q3 * R[:wy, :] + q4 * R[1:wy + 1, :]
 
 
-# ---- a6/a7: DepthProblem::warping (:162-191) and operator() for LSnorm = Tdist (:34-160)
-def depth_residual(rho, coor, T_left_virtual, Pl, Pr, ts_l, ts_r, wx, wy, nu, scale):
+# ---- a6/a7: DepthProblem::warping (:162-191) and operator() (:34-160) for LSnorm = Tdist, l2 and zncc
+def depth_residual(rho, coor, T_left_virtual, Pl, Pr, ts_l, ts_r, wx, wy, nu, scale, norm="Tdist", info=None):
+    """info (dict, optional) receives failed (the warp or the interpolation failed), trips (passes of the Tdist scale loop)
+    and margin (the smallest |change / 0.05 - 1| the loop's 5 % test saw: where it is at rounding level, a last-bit
+    difference of the residuals can change the number of passes and with it the whole vector)."""
     n = wx * wy
+    if info is not None:
+        info.update(failed=True, trips=0, margin=np.inf)
     H, W = ts_l.shape
 
-    def fail():
+    def fail():                                                                  # :43-59, :141-158
+        if norm == "l2":
+            return np.full(n, 255.0)
+        if norm == "zncc":
+            return np.full(n, 2 / np.sqrt(n))
         w = (nu + 1) / (nu + (255.0 / scale) ** 2)
         return np.full(n, np.sqrt(w) * 255.0)
     p_rv = cam2world(Pl, coor, rho)
@@ -83,6 +92,16 @@ def depth_residual(rho, coor, T_left_virtual, Pl, Pr, ts_l, ts_r, wx, wy, nu, sc
     t2 = patch_interpolation(ts_r, x2, wx, wy) if t1 is not None else None
     if t1 is None or t2 is None:
         return fail()
+    if info is not None:
+        info["failed"] = False
+    if norm == "l2":                                                             # :67-75
+        return (t1 - t2).ravel()
+    if norm == "zncc":                                                           # :76-87, tools::meanStdDev (utils.h:74-82)
+        def standardise(t):
+            mu = t.sum() / n
+            sigma = np.sqrt(((t - mu) ** 2).sum() / n) + 1e-6
+            return (t - mu) / sigma
+        return ((standardise(t1) - standardise(t2)) / np.sqrt(n)).ravel()
     r = (t1 - t2).ravel(); r2 = r * r
     s1, s2, first = scale * scale, -1.0, True
     while first or abs(s2 - s1) / s1 > 0.05:                                    # :96
@@ -96,6 +115,9 @@ def depth_residual(rho, coor, T_left_virtual, Pl, Pr, ts_l, ts_r, wx, wy, nu, sc
             break
         s2 = tot / n
         first = False
+        if info is not None:
+            info["trips"] += 1
+            info["margin"] = min(info["margin"], abs(abs(s2 - s1) / s1 / 0.05 - 1.0))
     with np.errstate(over="ignore", divide="ignore"):
         w = (nu + 1) / (nu + r2 / s2)
     return np.sqrt(w) * r
@@ -444,9 +466,11 @@ def time_surface_backward(ev, T_ns, decay_ms, W, H, ignore_polarity, median_blur
 
 
 # ---- a4: EventBM::match_an_event / match_all_HyperThread / match (esvo_core/src/core/EventBM.cpp:80-168,269-315) ----
-def event_bm_match_all(ev, ts_l, ts_r, lut_l, mask_l, pose_t, poses, wx, wy, dmin, dmax, step, thr, baseline, P00, num_thread):
+def event_bm_match_all(ev, ts_l, ts_r, lut_l, mask_l, pose_t, poses, wx, wy, dmin, dmax, step, thr, baseline, P00, num_thread,
+                       updown=False):
     """ev: dict x, y, t of the events handed to createMatchProblem (left camera, raw pixels).  Returns the EventMatchPairs (dicts)
-    in the reference's thread-major order and the number of zncc evaluations.  Left-right rig only (bUpDownConfiguration false)."""
+    in the reference's thread-major order and the number of zncc evaluations.  updown: bUpDownConfiguration_, the right camera
+    below the left one -- the search walks up the column instead of left along the row (:148-151, :181-184)."""
     H, W = ts_l.shape
     hx, hy = (wx - 1) // 2, (wy - 1) // 2
     tsl = ts_l.astype(np.float64); tsr = ts_r.astype(np.float64)
@@ -461,11 +485,11 @@ def event_bm_match_all(ev, ts_l, ts_r, lut_l, mask_l, pose_t, poses, wx, wy, dmi
         costs = {}
         d = start
         while d <= end:
-            x2 = x1[0] - d
-            if not valid(x2, x1[1]):
+            x2 = (x1[0], x1[1] - d) if updown else (x1[0] - d, x1[1])
+            if not valid(*x2):
                 costs[d] = 1.0
             else:
-                c = zncc_cost(patch, tsr[x1[1] - hy:x1[1] + hy + 1, x2 - hx:x2 + hx + 1])
+                c = zncc_cost(patch, tsr[x2[1] - hy:x2[1] + hy + 1, x2[0] - hx:x2[0] + hx + 1])
                 evals += 1
                 costs[d] = c
                 if c <= state["min"]:
@@ -488,19 +512,21 @@ def event_bm_match_all(ev, ts_l, ts_r, lut_l, mask_l, pose_t, poses, wx, wy, dmi
         patch = tsl[x1[1] - hy:x1[1] + hy + 1, x1[0] - hx:x1[0] + hx + 1]
         if (patch < 1).sum() > 0.95 * patch.size:                      # low information-to-noise ratio (:104-109)
             return None
-        st = dict(min=1.0, bx=0, bd=0)
+        st = dict(min=1.0, bx=(0, 0), bd=0)
         if not search(x1, patch, dmin, dmax, step, st):                # coarse
             return None
-        if not search(x1, patch, st["bd"] - (step - 1), st["bd"] + (step - 1), 1, st):     # fine
+        # fine (:128-131): the start bestDisp - (step - 1) is a size_t; below 0 it wraps to a huge value and the loop is empty
+        start = st["bd"] - (step - 1)
+        if not search(x1, patch, start if start >= 0 else 2 ** 64 + start, st["bd"] + (step - 1), 1, st):
             return None
         if not st["min"] <= thr:
             return None
-        disparity = float(x1[0] - st["bx"])
+        disparity = float(x1[1] - st["bx"][1]) if updown else float(x1[0] - st["bx"][0])
         k = int(np.searchsorted(pose_sec, ros_to_sec(ev["t"][i]), side="left"))             # StampTransformationMap_lower_bound on toSec()
         if k == len(pose_t):
             return None
         depth = baseline * P00 / disparity
-        return dict(i=i, x_left_raw=(float(ev["x"][i]), float(ev["y"][i])), x_left=xr, x_right=(float(st["bx"]), float(x1[1])), t_ns=int(ev["t"][i]),
+        return dict(i=i, x_left_raw=(float(ev["x"][i]), float(ev["y"][i])), x_left=xr, x_right=(float(st["bx"][0]), float(st["bx"][1])), t_ns=int(ev["t"][i]),
                     pose=k, inv_depth=1.0 / depth, cost=st["min"], disp=disparity)
 
     out = []

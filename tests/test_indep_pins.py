@@ -15,7 +15,7 @@ import pytest
 
 import indep_numpy as ind
 from esvo_b200 import capi, configs
-from util import build_ts_pair, scenario
+from util import FOLD_LENGTHS, build_ts_pair, fold_replay, fold_vector, grid_vs_map, scenario
 
 scipy_opt = pytest.importorskip("scipy.optimize")
 
@@ -34,6 +34,26 @@ def frame(oracle_lib):
     seeds, _ = o.bm_match(sd["x"], sd["y"], sd["t"], s["pose_t"], s["poses"])
     cams = configs.rig_arrays(RIG)
     return dict(o=o, s=s, tl=tl, tr=tr, seeds=seeds, prm=prm, Pl=cams["left"]["P"], Pr=cams["right"]["P"], d=o.get_derived())
+
+
+@pytest.fixture(scope="module")
+def shaped(frame, oracle_lib, request):
+    """The golden frame seen by an oracle context made with other parameters (request.param: patch shape, norm, search range,
+    step, rig orientation) on the same time surfaces; the default 15 x 7 seeds stay (a seed does not depend on the shape)."""
+    l, r = configs.rig_calibs(RIG)
+    prm = configs.params_for(RIG, oracle_lib)
+    for k, v in request.param.items():
+        setattr(prm, k, v)
+    o = capi.Backend(oracle_lib, l, r, prm)
+    o.set_ts_pair(frame["tl"], frame["tr"], frame["s"]["T_world_left"])
+    return dict(frame, o=o, prm=prm, d=o.get_derived())
+
+
+NORMS = {capi.LSNORM_TDIST: "Tdist", capi.LSNORM_L2: "l2", capi.LSNORM_ZNCC: "zncc"}
+
+
+def _shape_id(kw):
+    return "-".join(f"{k}={v}" for k, v in kw.items())
 
 
 def test_bm_cost_and_disparity_vs_numpy(frame):
@@ -58,15 +78,33 @@ def test_event_bm_accept_set_and_order_vs_numpy(frame):
     """a4: which events EventBM accepts (image bounds, mask, patch validity, the 95 % low-information rule, coarse / fine search,
     threshold, pose look-up), in which ORDER they come out (4 interleaved threads, results concatenated per thread) and every field
     of the EventMatchPair -- the oracle against tests/indep_numpy.py::event_bm_match_all, written from EventBM.cpp independently."""
-    f = frame
+    _check_event_bm_accept_set(frame, 400)
+
+
+BM_SHAPES = [dict(patch_size_x=5, patch_size_y=5), dict(patch_size_x=7, patch_size_y=15), dict(bm_updown=1),
+             dict(bm_step=3, bm_min_disparity=0, invdepth_min_range=0.01)]       # dmin = 0: the fine-search start wraps below 0
+
+
+@pytest.mark.parametrize("shaped,floor", [(kw, fl) for kw, fl in zip(BM_SHAPES, (500, 400, 40, 200))], indirect=["shaped"],
+                         ids=[_shape_id(kw) for kw in BM_SHAPES])
+def test_event_bm_accept_set_at_other_shapes_vs_numpy(shaped, floor):
+    """a4 off the shipped 15 x 7 left-right search: other patch shapes, the up-down rig (the search walks up the column) and a
+    coarse-to-fine search from disparity 0."""
+    if shaped["prm"].bm_step > 1:
+        assert shaped["d"]["min_disparity"] == 0
+    _check_event_bm_accept_set(shaped, floor)
+
+
+def _check_event_bm_accept_set(f, floor):
     o, s, prm = f["o"], f["s"], f["prm"]
     sd = s["seeds"]
     _, _, lut, mask = o.get_rectify_tables(0)
     d = f["d"]
     ref, evals = ind.event_bm_match_all(sd, f["tl"], f["tr"], lut, mask, s["pose_t"], s["poses"], prm.patch_size_x, prm.patch_size_y, d["min_disparity"],
-                                        d["max_disparity"], prm.bm_step, prm.bm_zncc_threshold, d["baseline"], f["Pl"][0, 0], prm.num_thread_mapping)
+                                        d["max_disparity"], prm.bm_step, prm.bm_zncc_threshold, d["baseline"], f["Pl"][0, 0], prm.num_thread_mapping,
+                                        updown=bool(prm.bm_updown))
     seeds, evals_o = o.bm_match(sd["x"], sd["y"], sd["t"], s["pose_t"], s["poses"])
-    assert len(ref) == seeds.size and len(ref) > 400, (len(ref), seeds.size)
+    assert len(ref) == seeds.size and len(ref) > floor, (len(ref), seeds.size)
     assert evals == evals_o
     for q, m in zip(seeds, ref):
         assert q["t_ns"] == m["t_ns"] and tuple(q["x_left_raw"]) == m["x_left_raw"]
@@ -235,8 +273,25 @@ def _oracle_residual(f, sd, rho):
 
 
 def test_depth_residual_vs_numpy(frame):
-    f = frame
+    _check_depth_residual(frame)
+
+
+RESIDUAL_SHAPES = [dict(patch_size_x=wx, patch_size_y=wy) for wx, wy in ((1, 1), (3, 3), (1, 15), (11, 11), (127, 1))]
+RESIDUAL_SHAPES += [dict(lsnorm=norm, patch_size_x=wx, patch_size_y=wy) for norm in (capi.LSNORM_L2, capi.LSNORM_ZNCC) for wx, wy in ((15, 7), (11, 11))]
+
+
+@pytest.mark.parametrize("shaped", RESIDUAL_SHAPES, indirect=True, ids=[_shape_id(kw) for kw in RESIDUAL_SHAPES])
+def test_depth_residual_at_other_shapes_vs_numpy(shaped):
+    """a6 at patch shapes of one pixel, one row, one column and up to 127 pixels, and for the l2 and zncc norms (whose
+    failure value 2 / sqrt(N) and scaling 1 / sqrt(N) depend on the shape)."""
+    _check_depth_residual(shaped)
+
+
+def _check_depth_residual(f):
     prm = f["prm"]
+    n = prm.patch_size_x * prm.patch_size_y
+    fail = {"l2": 255.0, "zncc": 2 / np.sqrt(n),                                 # the failed-warp value (DepthProblem.cpp:43-59)
+            "Tdist": np.sqrt((prm.td_nu + 1) / (prm.td_nu + (255.0 / prm.td_scale) ** 2)) * 255.0}[NORMS[prm.lsnorm]]
     rng = np.random.default_rng(1)
     pick = rng.choice(f["seeds"].size, 120, replace=False)
     worst = 0.0
@@ -244,17 +299,18 @@ def test_depth_residual_vs_numpy(frame):
     for k in pick:
         sd = f["seeds"][k]
         T = _T_left_virtual(f, sd)
-        for scale in (1.0, 1.013, 0.97):
+        for scale in (1.0, 1.013, 0.97, 6.0):            # 6 x the matched inverse depth warps some patches off the image
             rho = sd["inv_depth"] * scale
             a = ind.depth_residual(rho, sd["x_left"], T, f["Pl"], f["Pr"], f["tl"], f["tr"], prm.patch_size_x, prm.patch_size_y,
-                                   prm.td_nu, prm.td_scale)
+                                   prm.td_nu, prm.td_scale, NORMS[prm.lsnorm])
             b = _oracle_residual(f, sd, rho)
-            n_fail += np.all(a == a[0])
+            n_fail += np.all(a == fail)
             err = np.abs(a - b).max() / max(1.0, np.abs(b).max())
             worst = max(worst, err)
             assert err < 1e-9, (k, scale, err)
-    print("depth residual: worst rel deviation numpy vs oracle", worst, "constant (failed-warp) vectors", n_fail)
-    assert n_fail < 0.5 * 3 * pick.size
+    print(f"depth residual {prm.patch_size_x}x{prm.patch_size_y} {NORMS[prm.lsnorm]}: worst rel deviation numpy vs oracle {worst:.2e}, "
+          f"failed-warp vectors {n_fail}")
+    assert 0 < n_fail < 0.5 * 4 * pick.size
 
 
 def test_minpack_on_depth_problem_vs_oracle_solve(frame):
@@ -267,7 +323,17 @@ def test_minpack_on_depth_problem_vs_oracle_solve(frame):
         the forward-difference Jacobian amplifies: 1e-6 relative = xtol);
       * the oracle's final rho (after the extra steps) stays within the solver tolerance of it;
       * the variance td_stdvar^2 / (J^T J) (:207-211) agrees with MINPACK's covariance at the solution."""
-    f = frame
+    _check_minpack(frame)
+
+
+@pytest.mark.parametrize("shaped", [dict(patch_size_x=3, patch_size_y=3), dict(patch_size_x=11, patch_size_y=11)], indirect=True,
+                         ids=["3x3", "11x11"])
+def test_minpack_on_depth_problem_at_other_shapes_vs_oracle_solve(shaped):
+    """a9 with 9 and 121 residuals per seed (the shipped 105 sits between them)."""
+    _check_minpack(shaped)
+
+
+def _check_minpack(f):
     prm = f["prm"]
     seeds = f["seeds"]
     pts_o, _ = f["o"].depth_solve(seeds)
@@ -393,20 +459,6 @@ def test_time_surface_backward_vs_numpy_and_cv2(oracle_lib, rig, polarity, media
         assert ts.max() > 0
 
 
-def _grid_vs_map(grid, m, tag):
-    assert len(grid.elements) == m.size, (tag, len(grid.elements), m.size)
-    assert [e.row for e in grid.elements] == m["row"].tolist() and [e.col for e in grid.elements] == m["col"].tolist(), tag + ": element order"
-    assert [e.age for e in grid.elements] == m["age"].tolist(), tag + ": ages"
-    for name, get in (("inv_depth", lambda e: e.rho), ("scale2", lambda e: e.s2), ("nu", lambda e: e.nu), ("variance", lambda e: e.var),
-                      ("residual", lambda e: e.res)):
-        a = np.array([get(e) for e in grid.elements]); b = m[name]
-        assert np.allclose(a, b, rtol=1e-10, atol=1e-300), (tag, name, np.abs(a - b).max())
-    pc = np.array([e.p_cam for e in grid.elements])
-    assert np.allclose(pc, m["p_cam"], rtol=1e-9, atol=1e-12), tag + ": p_cam"
-    xx = np.array([e.x for e in grid.elements])
-    assert np.allclose(xx, m["x"], rtol=1e-12, atol=0), tag + ": x"
-
-
 @pytest.mark.parametrize("radii", [(0, 0, 1), (1, 0, 1)])
 def test_fusion_case_analysis_clean_and_regularisation_vs_python(frame, radii):
     """The map-side control flow -- DepthFusion::update / fusion with its four cases (create, compatible fuse, occlusion,
@@ -441,18 +493,18 @@ def test_fusion_case_analysis_clean_and_regularisation_vs_python(frame, radii):
         nf_p = inf.fuse_vector(grid, vec, T0, f["Pl"], W, H, radius)
         n_rep += sum(1 for e in grid.elements if id(e) in before and before[id(e)] != (e.row, e.col))
         assert nf_o == nf_p, (k, nf_o, nf_p)
-        _grid_vs_map(grid, o.map_download(), f"round {k}")
+        grid_vs_map(grid, o.map_download(), f"round {k}")
     assert n_rep > 0, "the replace branch (case 2.2, dm->get(row,col) = dp_prop) was never taken"
     o.map_clean(prm.stdvar_vis_threshold ** 2, prm.age_vis_threshold, prm.invdepth_max_range, prm.invdepth_min_range)
     n_before = len(grid.elements)
     grid.clean(prm.stdvar_vis_threshold ** 2, prm.age_vis_threshold, prm.invdepth_max_range, prm.invdepth_min_range)
     assert len(grid.elements) < n_before
-    _grid_vs_map(grid, o.map_download(), "clean")
+    grid_vs_map(grid, o.map_download(), "clean")
     o.map_regularize()
     m = o.map_download()
     # (a) keyed by the cell that holds the element -- the oracle's and the kernels' documented choice (DESIGN.md deviation 7)
     grid2 = inf.regularize(grid, prm.reg_radius, prm.reg_min_neighbours, prm.reg_min_close_neighbours, literal=False)
-    _grid_vs_map(grid2, m, "regularise")
+    grid_vs_map(grid2, m, "regularise")
     assert (m["inv_depth"] == -1.0).any() and (m["inv_depth"] > 0).any()
     # (b) exactly as written: an element whose row_/col_ a replacement copied from another pixel is keyed by the cell it NAMES,
     # i.e. merged into that cell while its own cell vanishes.  The two differ by those elements only.
@@ -468,6 +520,42 @@ def test_fusion_case_analysis_clean_and_regularisation_vs_python(frame, radii):
         assert grid3.cell[k].rho == grid2.cell[k].rho, k
     print("regularisation: %d elements, %d with copied coordinates, literal reading merges %d" %
           (len(grid2.elements), len(moved), len(grid2.elements) - len(grid3.elements)))
+
+
+@pytest.mark.parametrize("mode", ["radius0", "radius1", "naive"])
+def test_fold_at_chosen_list_lengths_vs_python(oracle_lib, mode):
+    """The hand-built fold vector of util.fold_vector (lists of 1 .. 500 contributions per pixel, interleaved): the oracle
+    against tests/indep_fusion.py, and the vector has teeth -- every target pixel gets exactly its list length, and replaying
+    the same points in reverse order changes the surviving element of the pixels, so an order mistake in a replay shows."""
+    l, r = configs.rig_calibs(RIG)
+    o = capi.Backend(oracle_lib, l, r, configs.params_for(RIG, oracle_lib))
+    Pl = configs.rig_arrays(RIG)["left"]["P"]
+    pts, targets = fold_vector(Pl)
+    assert [t[2] for t in targets] == list(FOLD_LENGTHS)
+    x = np.array([Pl[:2, :3] @ q["p_cam"] / (Pl[2, :3] @ q["p_cam"]) for q in pts])      # identity poses: where each point lands
+    landed = {}
+    for c, rw in np.floor(x).astype(int):
+        landed[(rw, c)] = landed.get((rw, c), 0) + 1
+    assert landed == {(rw, c): L for rw, c, L in targets}
+    radius = 1 if mode == "radius1" else 0
+    naive = mode == "naive"
+    if naive:
+        o.naive_propagate(pts, np.eye(4), True); nf = 0
+    else:
+        nf = o.fuse(pts, np.eye(4), radius, True)
+    stats = {}
+    grid, nfp = fold_replay(pts, Pl, o.W, o.H, radius, naive=naive, stats=stats)
+    print(mode, "branch outcomes of the replay:", stats)
+    assert nf == nfp and (naive or nf > 4000)
+    assert min(stats.values()) >= 10 and len(stats) == (4 if naive else 5), stats    # every branch of the case analysis is taken
+    grid_vs_map(grid, o.map_download(), mode)
+    rev, _ = fold_replay(pts[::-1], Pl, o.W, o.H, radius, naive=naive)
+    changed = [L for rw, c, L in targets if (grid.cell[(rw, c)].rho, grid.cell[(rw, c)].age) != (rev.cell[(rw, c)].rho, rev.cell[(rw, c)].age)]
+    print(mode, "pixels whose element the reversed replay changes:", changed)
+    if naive:      # an occupied pixel only takes a nearer point with a smaller residual: fewer pixels depend on the order
+        assert len(changed) >= 8
+    else:
+        assert changed == [L for L in FOLD_LENGTHS if L > 1]
 
 
 def test_tracking_residual_and_jacobian_vs_numpy(frame):
