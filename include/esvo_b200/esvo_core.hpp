@@ -12,6 +12,7 @@
 #include <array>
 #include <cmath>
 #include <cstdint>
+#include <cstdio>
 #include <deque>
 #include <functional>
 #include <map>
@@ -64,6 +65,36 @@ struct TimeSurfaceObservation {
   void setTransformation(const Pose& tr) { tr_ = tr; }
 };
 using StampedTimeSurfaceObs = std::pair<int64_t, TimeSurfaceObservation>;
+
+// Eigen::Quaterniond(const Matrix3d&) (Eigen/src/Geometry/Quaternion.h, quaternion_assign_impl): R row-major 3x3, q = x, y, z, w
+inline void quaternionFromRotation(const double R[9], double q[4]) {
+  auto m = [&](int r, int c) { return R[3 * r + c]; };
+  double t = m(0, 0) + m(1, 1) + m(2, 2);
+  if (t > 0) {
+    t = std::sqrt(t + 1.0);
+    q[3] = 0.5 * t;
+    t = 0.5 / t;
+    q[0] = (m(2, 1) - m(1, 2)) * t; q[1] = (m(0, 2) - m(2, 0)) * t; q[2] = (m(1, 0) - m(0, 1)) * t;
+  } else {
+    int i = 0;
+    if (m(1, 1) > m(0, 0)) i = 1;
+    if (m(2, 2) > m(i, i)) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    t = std::sqrt(m(i, i) - m(j, j) - m(k, k) + 1.0);
+    q[i] = 0.5 * t;
+    t = 0.5 / t;
+    q[3] = (m(k, j) - m(j, k)) * t; q[j] = (m(j, i) + m(i, j)) * t; q[k] = (m(k, i) + m(i, k)) * t;
+  }
+}
+// QuaternionBase::toRotationMatrix (same file): q = x, y, z, w -> R row-major 3x3 (no normalisation)
+inline void rotationFromQuaternion(const double q[4], double R[9]) {
+  const double x = q[0], y = q[1], z = q[2], w = q[3];
+  const double tx = 2 * x, ty = 2 * y, tz = 2 * z;
+  const double twx = tx * w, twy = ty * w, twz = tz * w, txx = tx * x, txy = ty * x, txz = tz * x, tyy = ty * y, tyz = tz * y, tzz = tz * z;
+  R[0] = 1 - (tyy + tzz); R[1] = txy - twz; R[2] = txz + twy;
+  R[3] = txy + twz; R[4] = 1 - (txx + tzz); R[5] = tyz - twx;
+  R[6] = txz - twy; R[7] = tyz + twx; R[8] = 1 - (txx + tyy);
+}
 
 }  // namespace esvo
 
@@ -327,7 +358,8 @@ inline int64_t fromSec(double t) {   // ros::Time(double): sec = floor(t), nsec 
   sec += nsec / 1000000000LL; nsec %= 1000000000LL;
   return sec * 1000000000LL + nsec;
 }
-inline void selectCloseEvents(std::vector<esvo::Event>& events_left /* time-ordered */, int64_t t_end_ns, double BM_half_slice_thickness,
+template <class EventBuffer>
+inline void selectCloseEventsIn(EventBuffer& events_left /* time-ordered */, int64_t t_end_ns, double BM_half_slice_thickness,
                               size_t PROCESS_EVENT_NUM, std::vector<esvo::Event*>& vCloseEventsPtr_left) {
   vCloseEventsPtr_left.clear();
   if (events_left.empty()) return;
@@ -354,7 +386,8 @@ inline void selectCloseEvents(std::vector<esvo::Event>& events_left /* time-orde
 }
 //  * selectSGMEvents: the INITIALIZATION branch of dataTransferring (:538-552) -- window 2*BM_half_slice_thickness and
 //    `<=` instead of `<` on the count (one event more than PROCESS_EVENT_NUM).
-inline void selectSGMEvents(std::vector<esvo::Event>& events_left, int64_t t_end_ns, double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM,
+template <class EventBuffer>
+inline void selectSGMEventsIn(EventBuffer& events_left, int64_t t_end_ns, double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM,
                             std::vector<esvo::Event*>& vEventsPtr_left_SGM) {
   vEventsPtr_left_SGM.clear();
   if (events_left.empty()) return;
@@ -370,6 +403,22 @@ inline void selectSGMEvents(std::vector<esvo::Event>& events_left, int64_t t_end
   size_t budget = PROCESS_EVENT_NUM + 1;      // `<=` on the count: one event more than PROCESS_EVENT_NUM
   if (ev_end == events_left.size() && ev_end != ev_begin) { --ev_end; --budget; }   // skip the one-past-the-end slot (see selectCloseEvents)
   while (ev_end != ev_begin && vEventsPtr_left_SGM.size() < budget) { vEventsPtr_left_SGM.push_back(&events_left[ev_end]); --ev_end; }
+}
+inline void selectCloseEvents(std::vector<esvo::Event>& events_left /* time-ordered */, int64_t t_end_ns, double BM_half_slice_thickness,
+                              size_t PROCESS_EVENT_NUM, std::vector<esvo::Event*>& vCloseEventsPtr_left) {
+  selectCloseEventsIn(events_left, t_end_ns, BM_half_slice_thickness, PROCESS_EVENT_NUM, vCloseEventsPtr_left);
+}
+inline void selectCloseEvents(std::deque<esvo::Event>& events_left /* time-ordered: the node's EventQueue */, int64_t t_end_ns,
+                              double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM, std::vector<esvo::Event*>& vCloseEventsPtr_left) {
+  selectCloseEventsIn(events_left, t_end_ns, BM_half_slice_thickness, PROCESS_EVENT_NUM, vCloseEventsPtr_left);
+}
+inline void selectSGMEvents(std::vector<esvo::Event>& events_left, int64_t t_end_ns, double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM,
+                            std::vector<esvo::Event*>& vEventsPtr_left_SGM) {
+  selectSGMEventsIn(events_left, t_end_ns, BM_half_slice_thickness, PROCESS_EVENT_NUM, vEventsPtr_left_SGM);
+}
+inline void selectSGMEvents(std::deque<esvo::Event>& events_left, int64_t t_end_ns, double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM,
+                            std::vector<esvo::Event*>& vEventsPtr_left_SGM) {
+  selectSGMEventsIn(events_left, t_end_ns, BM_half_slice_thickness, PROCESS_EVENT_NUM, vEventsPtr_left_SGM);
 }
 inline std::vector<int64_t> samplePoseStamps(int64_t t_end_ns, double BM_half_slice_thickness) {
   std::vector<int64_t> out;
@@ -498,8 +547,150 @@ class esvo_Mapping {
     return InitializationAtTime(TS_obs, disp.data(), vEventsPtr_left_SGM, INIT_SGM_DP_NUM_Threshold, n_points);
   }
   void reset() { esvo_mapping_reset(cs_->ctx()); }
+
+  // ---- the node around MappingAtTime / InitializationAtTime: callbacks, dataTransferring and one pass of MappingLoop ----
+  // (esvo_Mapping.cpp:179-259,494-605,669-762).  The ROS subscriptions become plain methods that fill the same buffers; the
+  // tf look-up becomes a pose provider; ESVO_System_Status_ is the /ESVO_SYSTEM_STATUS value the owner keeps in sync.
+  using PoseProvider = std::function<bool(int64_t /*stamp ns*/, esvo::Pose& /*T_world_dvs*/)>;   // getPoseAt (:646-667)
+  void setPoseProvider(PoseProvider f) { getPoseAt_ = std::move(f); }
+  // node parameters (constructor defaults of esvo_Mapping.cpp:77-92; cfg/mapping/*.yaml override them)
+  size_t PROCESS_EVENT_NUM_ = 500, TS_HISTORY_LENGTH_ = 100, INIT_SGM_DP_NUM_Threshold_ = 500;
+  double BM_half_slice_thickness_ = 0.001;
+  bool bDenoising_ = false;
+  std::string ESVO_System_Status_ = "INITIALIZATION";
+  // eventsCallback (:669-703) for events_left_ / events_right_: insertion-sorted, capped at 3e6
+  void eventsCallback(const std::vector<esvo::Event>& events, bool left) {
+    std::deque<esvo::Event>& EQ = left ? events_left_ : events_right_;
+    for (const esvo::Event& e : events) {
+      EQ.push_back(e);
+      long i = (long)EQ.size() - 2;
+      while (i >= 0 && EQ[(size_t)i].ts > e.ts) { EQ[(size_t)i + 1] = EQ[(size_t)i]; --i; }
+      EQ[(size_t)(i + 1)] = e;
+    }
+    static constexpr size_t MAX_EVENT_QUEUE_LENGTH = 3000000;
+    if (EQ.size() > MAX_EVENT_QUEUE_LENGTH) EQ.erase(EQ.begin(), EQ.begin() + (long)(EQ.size() - MAX_EVENT_QUEUE_LENGTH));
+  }
+  // timeSurfaceCallback (:716-762): the stereo pair is copied into a history of TS_HISTORY_LENGTH_ entries
+  void timeSurfaceCallback(int64_t stamp_ns, const uint8_t* time_surface_left, const uint8_t* time_surface_right) {
+    const size_t n = (size_t)cs_->width_ * cs_->height_;
+    TS_history_[stamp_ns] = TsPair{std::vector<uint8_t>(time_surface_left, time_surface_left + n),
+                                   std::vector<uint8_t>(time_surface_right, time_surface_right + n), TS_id_++};
+    while (TS_history_.size() > TS_HISTORY_LENGTH_) TS_history_.erase(TS_history_.begin());
+  }
+  // dataTransferring (:494-605).  Leaves TS_obs_ (second-newest entry with a pose; identity in INITIALIZATION), and
+  // vEventsPtr_left_SGM_ (INITIALIZATION) or vALLEventsPtr_left_ / vCloseEventsPtr_left_ / st_map_ (WORKING).
+  bool dataTransferring() {
+    TS_obs_ = esvo::StampedTimeSurfaceObs(); has_obs_ = false;
+    if (TS_history_.size() <= 10) return false;
+    auto it_end = TS_history_.rbegin();
+    ++it_end;                                             // in case the tf is behind the most current TS
+    const int64_t t_oldest = TS_history_.begin()->first;
+    while (!has_obs_) {
+      esvo::Pose tr{};
+      if (ESVO_System_Status_ == "INITIALIZATION") { tr = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}; has_obs_ = true; }
+      if (ESVO_System_Status_ == "WORKING") {
+        if (getPoseAt_ && getPoseAt_(it_end->first, tr)) has_obs_ = true;
+        else if (ESVO_System_Status_ != "WORKING") return false;
+      }
+      if (has_obs_) {
+        TS_obs_.first = it_end->first;
+        TS_obs_.second.left = it_end->second.left.data(); TS_obs_.second.right = it_end->second.right.data();
+        TS_obs_.second.id_ = it_end->second.id; TS_obs_.second.setTransformation(tr);
+      }
+      if (it_end->first == t_oldest) break;
+      ++it_end;
+    }
+    if (!has_obs_) return false;
+    if (ESVO_System_Status_ == "INITIALIZATION")           // SGM (:537-552)
+      frontend::selectSGMEvents(events_left_, TS_obs_.first, BM_half_slice_thickness_, PROCESS_EVENT_NUM_, vEventsPtr_left_SGM_);
+    if (ESVO_System_Status_ == "WORKING") {                // BM (:554-603)
+      frontend::selectCloseEvents(events_left_, TS_obs_.first, BM_half_slice_thickness_, PROCESS_EVENT_NUM_, vCloseEventsPtr_left_);
+      vALLEventsPtr_left_ = vCloseEventsPtr_left_;         // both are filled by the same walk (:569-574)
+      st_map_.clear();
+      for (int64_t t : frontend::samplePoseStamps(TS_obs_.first, BM_half_slice_thickness_)) {
+        esvo::Pose tr;
+        if (getPoseAt_ && getPoseAt_(t, tr)) st_map_.push_back({t, tr});
+        else if (ESVO_System_Status_ != "WORKING") return false;
+      }
+    }
+    return true;
+  }
+  // What one pass of MappingLoop did.  ran: 0 nothing, 1 InitializationAtTime, 2 MappingAtTime; ok: the call's result;
+  // cloud: the local map as publishPointCloud publishes it (world frame, at the observation's pose), if it did.
+  struct LoopResult {
+    int ran = 0; bool ok = false; size_t n_sgm_points = 0; Counters ctr{};
+    bool published = false; int64_t stamp = 0; esvo::Pose T_world_obs{}; std::vector<float> cloud;
+  };
+  // one pass of MappingLoop's body (:194-248) with publishMappingResults / publishPointCloud (:396-403,488-490,868-953) run in line
+  bool MappingLoopOnce(LoopResult& res) {
+    res = LoopResult();
+    if (ESVO_System_Status_ == "TERMINATE" || TS_history_.size() < 10) return false;
+    dataTransferring();
+    if (!has_obs_) return false;
+    if (ESVO_System_Status_ == "INITIALIZATION" || ESVO_System_Status_ == "RESET") {
+      res.ran = 1;
+      res.ok = InitializationAtTime(TS_obs_, vEventsPtr_left_SGM_, INIT_SGM_DP_NUM_Threshold_, &res.n_sgm_points);
+      if (res.ok) publishMappingResults(res);
+    }
+    if (ESVO_System_Status_ == "WORKING") {
+      res.ran = 2;
+      vDenoisedEventsPtr_left_.clear();
+      if (bDenoising_) {                                   // :282-296
+        std::vector<uint8_t> mask;
+        frontend::createDenoisingMask(vALLEventsPtr_left_, mask, (size_t)cs_->height_, (size_t)cs_->width_);
+        frontend::extractDenoisedEvents(vCloseEventsPtr_left_, vDenoisedEventsPtr_left_, mask, (size_t)cs_->width_, PROCESS_EVENT_NUM_);
+      } else {                                             // :297-304
+        vDenoisedEventsPtr_left_.assign(vCloseEventsPtr_left_.begin(),
+                                        vCloseEventsPtr_left_.begin() + (long)std::min(vCloseEventsPtr_left_.size(), PROCESS_EVENT_NUM_));
+      }
+      res.ok = MappingAtTime(TS_obs_, vDenoisedEventsPtr_left_, st_map_, &res.ctr);
+      if (res.ok) publishMappingResults(res);
+    }
+    return res.ok;
+  }
+  // Number of vectors in the fusion window (dqvDepthPoints_.size()) and of points in them, read from the ctx.
+  size_t fusionWindow(size_t* n_points = nullptr) {
+    size_t k = 0, total = 0;
+    for (;; ++k) {
+      size_t n = 0;
+      const int rc = esvo_window_download(cs_->ctx(), (int)k, nullptr, &n);
+      if (rc != ESVO_OK && rc != ESVO_ERR_CAPACITY) break;
+      total += n;
+    }
+    if (n_points) *n_points = total;
+    return k;
+  }
+  esvo::StampedTimeSurfaceObs TS_obs_;
+  std::vector<esvo::Event*> vEventsPtr_left_SGM_, vALLEventsPtr_left_, vCloseEventsPtr_left_, vDenoisedEventsPtr_left_;
+  esvo::StampTransformationMap st_map_;
  private:
+  // publishMappingResults (:868-907): in INITIALIZATION always, in WORKING once the fusion window is full (CONST_FRAMES) or
+  // holds more than half of maxNumFusionPoints (CONST_POINTS); publishPointCloud (:909-953) skips an empty cloud
+  void publishMappingResults(LoopResult& res) {
+    const esvo_params& p = cs_->params();
+    bool publish = ESVO_System_Status_ == "INITIALIZATION";
+    if (ESVO_System_Status_ == "WORKING") {
+      size_t n_points = 0;
+      const size_t n_frames = fusionWindow(&n_points);
+      if (p.fusion_strategy == ESVO_FUSION_CONST_FRAMES) publish = n_frames == (size_t)p.max_num_fusion_frames;
+      else publish = (double)n_points > 0.5 * (double)p.max_num_fusion_points;
+    }
+    if (!publish) return;
+    std::vector<esvo::DepthPoint> elems((size_t)cs_->width_ * cs_->height_);
+    size_t n = elems.size();
+    if (esvo_map_download(cs_->ctx(), elems.data(), &n) != ESVO_OK) n = 0;
+    elems.resize(n);
+    frontend::packPointCloud(elems, TS_obs_.second.tr_, res.cloud);
+    if (res.cloud.empty()) return;
+    res.published = true; res.stamp = TS_obs_.first; res.T_world_obs = TS_obs_.second.tr_;
+  }
+  struct TsPair { std::vector<uint8_t> left, right; size_t id; };
   esvo::CameraSystem::Ptr cs_;
+  std::deque<esvo::Event> events_left_, events_right_;   // EventQueue (esvo_Mapping.h)
+  std::map<int64_t, TsPair> TS_history_;
+  size_t TS_id_ = 0;
+  bool has_obs_ = false;
+  PoseProvider getPoseAt_;
 };
 
 // esvo_core::esvo_MVStereo::MappingAtTime (esvo_MVStereo.cpp:239-520): the known-pose multi-view-stereo node the reference
@@ -707,16 +898,19 @@ class esvo_Tracking {
     if (ESVO_System_Status_ == "INITIALIZATION" && ets_ == WORKING) { reset(); return false; }
     if (ESVO_System_Status_ == "TERMINATE") return false;
     if (frontend::toSec(ref_.t_) < frontend::toSec(refPCMap_.rbegin()->first))            // new reference map arrived
-      if (!refDataTransferring()) return false;
+      if (!refDataTransferring()) { error_ = "no pose for the reference map"; return false; }
     if (frontend::toSec(cur_.t_) < frontend::toSec(TS_history_.rbegin()->first)) {          // new observation arrived
-      if (frontend::toSec(ref_.t_) >= frontend::toSec(TS_history_.rbegin()->first)) return false;   // obs must come after the ref (reference: exit(-1))
+      if (frontend::toSec(ref_.t_) >= frontend::toSec(TS_history_.rbegin()->first)) {       // obs must come after the ref (reference: exit(-1))
+        error_ = "time-surface observation is not newer than the reference map";
+        return false;
+      }
       if (!curDataTransferring()) return false;
     } else return false;
     if (rpSolver_.resetRegProblem(&ref_, &cur_)) {
       if (ets_ == IDLE) ets_ = WORKING;
       if (ESVO_System_Status_ != "WORKING") ESVO_System_Status_ = "WORKING";
       const bool ok = rpType_ == core::REG_NUMERICAL ? rpSolver_.solve_numerical() : rpSolver_.solve_analytical();
-      if (!ok) return false;
+      if (!ok) { error_ = std::string("tracking solve: ") + esvo_last_error(cs_->ctx()); return false; }   // device / ABI error only
       T_world_cur_ = cur_.tr_;
       lTimestamp_.push_back(cur_.t_); lPose_.push_back(cur_.tr_);                             // publishPose / saveTrajectory payload
       return true;
@@ -726,8 +920,28 @@ class esvo_Tracking {
     return false;
   }
   void reset() { ets_ = IDLE; TS_id_ = 0; TS_history_.clear(); refPCMap_.clear(); events_left_.clear(); }   // (:247-255)
+  // saveTrajectory (:430-462): per tracked frame "<std::to_string(t.toSec())> tx ty tz qx qy qz qw", fixed notation, precision 9
+  // after the stamp; q = Eigen::Quaterniond(R) (esvo::quaternionFromRotation).  The translation is written as Eigen's default
+  // IOFormat writes twc.transpose(): every column right-aligned to the widest of the three.  false if the file cannot be opened.
+  bool saveTrajectory(const std::string& path) const {
+    std::FILE* f = std::fopen(path.c_str(), "w");
+    if (!f) return false;
+    for (size_t i = 0; i < lPose_.size(); ++i) {
+      const esvo::Pose& T = lPose_[i];
+      const double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]};
+      double q[4];
+      esvo::quaternionFromRotation(R, q);
+      char t[3][64];
+      int w = 0;
+      for (int k = 0; k < 3; ++k) w = std::max(w, std::snprintf(t[k], sizeof(t[k]), "%.9f", T[4 * k + 3]));
+      std::fprintf(f, "%s %*s %*s %*s %.9f %.9f %.9f %.9f\n", std::to_string(frontend::toSec(lTimestamp_[i])).c_str(), w, t[0], w, t[1], w, t[2],
+                   q[0], q[1], q[2], q[3]);
+    }
+    return std::fclose(f) == 0;
+  }
 
   std::string ESVO_System_Status_ = "INITIALIZATION";   // the /ESVO_SYSTEM_STATUS parameter
+  std::string error_;                                  // set where the reference exit(-1)s; the pass then returned false
   TrackingStatus ets_ = IDLE;
   core::RefFrame ref_;
   core::CurFrame cur_;
