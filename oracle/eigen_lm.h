@@ -26,6 +26,7 @@ struct ColPivQR {
   std::vector<int> perm;      // perm[j] = original column at position j
   double maxpivot = 0;
   int nonzero_pivots = 0;
+  int downdate_recomputes = 0;   // trace only: columns whose norm the downdate re-computed instead of updating
   double& at(int i, int j) { return qr[(size_t)j * m + i]; }
   double at(int i, int j) const { return qr[(size_t)j * m + i]; }
 
@@ -48,6 +49,7 @@ struct ColPivQR {
     const double norm_downdate_threshold = std::sqrt(eps);
     nonzero_pivots = size;
     maxpivot = 0;
+    downdate_recomputes = 0;
     for (int k = 0; k < size; ++k) {
       int big = k;
       double bigv = normsUpdated[k];
@@ -101,6 +103,7 @@ struct ColPivQR {
             for (int i = k + 1; i < m; ++i) s += at(i, j) * at(i, j);
             normsDirect[j] = std::sqrt(s);
             normsUpdated[j] = normsDirect[j];
+            ++downdate_recomputes;
           } else {
             normsUpdated[j] *= std::sqrt(temp);
           }
@@ -198,10 +201,11 @@ static inline void qrsolv(std::vector<double>& s, int n, const std::vector<int>&
   for (int j = 0; j < n; ++j) x[ipvt[j]] = wa[j];
 }
 
-// internal::lmpar2
+// internal::lmpar2.  n_iter (optional, trace only) receives the number of passes of the par
+// iteration: 0 when the Gauss-Newton step already lies within 10 % of the trust region (par = 0).
 static inline void lmpar2(const ColPivQR& qr, const std::vector<double>& diag,
                           const std::vector<double>& qtb, double delta, double& par,
-                          std::vector<double>& x) {
+                          std::vector<double>& x, int* n_iter = nullptr) {
   const double dwarf = std::numeric_limits<double>::min();
   const int n = qr.n;
   std::vector<double> wa1(qtb.begin(), qtb.begin() + n), wa2(n);
@@ -218,6 +222,7 @@ static inline void lmpar2(const ColPivQR& qr, const std::vector<double>& diag,
   for (int j = 0; j < n; ++j) wa2[j] = diag[j] * x[j];
   double dxnorm = vnorm(wa2.data(), n);
   double fp = dxnorm - delta;
+  if (n_iter) *n_iter = 0;
   if (fp <= 0.1 * delta) { par = 0; return; }
   double parl = 0.;
   if (rank == n) {
@@ -270,6 +275,7 @@ static inline void lmpar2(const ColPivQR& qr, const std::vector<double>& diag,
     par = std::max(parl, par + parc);
   }
   if (iter == 0) par = 0.;
+  if (n_iter) *n_iter = iter;
 }
 
 enum LMStatus {
@@ -278,6 +284,20 @@ enum LMStatus {
   LM_RelativeErrorAndReductionTooSmall = 3, LM_CosinusTooSmall = 4,
   LM_TooManyFunctionEvaluation = 5, LM_FtolTooSmall = 6, LM_XtolTooSmall = 7,
   LM_GtolTooSmall = 8, LM_UserAsked = 9
+};
+
+// Optional record of one minimizeOneStep (test infrastructure: recording changes no arithmetic).
+struct LMStepTrace {
+  struct Trial {
+    std::vector<double> x;                       // the trial point x + p
+    double fnorm1, actred, prered, ratio;
+    double par, delta, xnorm;                    // after the trust-region update of this trial
+    bool accepted;
+    int lmpar_iter;                              // 0: lmpar returned early with par = 0
+  };
+  int rank = 0, nonzero_pivots = 0, downdate_recomputes = 0;
+  double fnorm = 0, gnorm = 0;                   // at the start of the step
+  std::vector<Trial> trials;
 };
 
 // f(x, fvec) -> <0 aborts;  df(x, fjac col-major m x n) -> number of f evaluations (numerical
@@ -294,6 +314,7 @@ struct LevenbergMarquardt {
   ColPivQR qrfac;
   int nfev = 0, njev = 0, iter = 0;
   double fnorm = 0, gnorm = 0, par = 0, xnorm = 0, delta = 0;
+  LMStepTrace* trace = nullptr;   // filled by minimizeOneStep when set
 
   LevenbergMarquardt() { ftol = xtol = std::sqrt(std::numeric_limits<double>::epsilon()); }
 
@@ -320,6 +341,11 @@ struct LevenbergMarquardt {
     qrfac.compute(fjac, m, n);
     fjac = qrfac.qr;
     const std::vector<int>& perm = qrfac.perm;
+    if (trace) {
+      *trace = LMStepTrace();
+      trace->rank = qrfac.rank(); trace->nonzero_pivots = qrfac.nonzero_pivots;
+      trace->downdate_recomputes = qrfac.downdate_recomputes; trace->fnorm = fnorm;
+    }
     if (iter == 1) {
       for (int j = 0; j < n; ++j) diag[j] = (wa2[j] == 0.) ? 1. : wa2[j];
       double s = 0;
@@ -339,11 +365,13 @@ struct LevenbergMarquardt {
           for (int i = 0; i <= j; ++i) s += qrfac.at(i, j) * (qtf[i] / fnorm);
           gnorm = std::max(gnorm, std::fabs(s / wa2[perm[j]]));
         }
+    if (trace) trace->gnorm = gnorm;
     if (gnorm <= gtol) return LM_CosinusTooSmall;
     for (int j = 0; j < n; ++j) diag[j] = std::max(diag[j], wa2[j]);
     double ratio;
     do {
-      lmpar2(qrfac, diag, qtf, delta, par, wa1);
+      int lmpar_iter = 0;
+      lmpar2(qrfac, diag, qtf, delta, par, wa1, &lmpar_iter);
       for (int j = 0; j < n; ++j) { wa1[j] = -wa1[j]; wa2[j] = x[j] + wa1[j]; }
       double s = 0;
       for (int j = 0; j < n; ++j) s += (diag[j] * wa1[j]) * (diag[j] * wa1[j]);
@@ -386,6 +414,9 @@ struct LevenbergMarquardt {
         fnorm = fnorm1;
         ++iter;
       }
+      if (trace)
+        trace->trials.push_back({ratio >= 1e-4 ? x : wa2, fnorm1, actred, prered, ratio, par, delta, xnorm,
+                                 ratio >= 1e-4, lmpar_iter});
       if (std::fabs(actred) <= ftol && prered <= ftol && .5 * ratio <= 1. && delta <= xtol * xnorm)
         return LM_RelativeErrorAndReductionTooSmall;
       if (std::fabs(actred) <= ftol && prered <= ftol && .5 * ratio <= 1.)

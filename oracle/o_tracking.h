@@ -118,6 +118,12 @@ struct RegProblem {
   size_t numPoints = 0, numBatches = 1;
   GlibcRand rng;
   uint64_t n_evals = 0;
+  // Trace of the last solve (test infrastructure), per outer iteration: TRACE_HEAD doubles {batch offset, m, status,
+  // nfev, rank, nonzero_pivots, norm-downdate recomputes, number of trials, fnorm, gnorm, R_[9], t_[3] (the state the
+  // iteration starts from)}, then per trial
+  // TRACE_TRIAL doubles {x[6], fnorm1, actred, prered, ratio, par, delta, xnorm, accepted, lmpar iterations}.
+  static constexpr int TRACE_HEAD = 22, TRACE_TRIAL = 15;
+  std::vector<double> trace;
 
   // computeJ_G at x = 0 (RegProblemLM.cpp:271-320): only J_G_0_ is ever used (:21).
   void init() {
@@ -282,12 +288,30 @@ struct RegProblem {
     else lm.df = [&](const std::vector<double>& x, std::vector<double>& J) { return numerical_diff_forward(lm.f, x, J, (int)numPoints); };
     lm.ftol = 1e-3; lm.xtol = 1e-3; lm.maxfev = prm.trk_max_iteration * 8;
     size_t iteration = 0, nfev = 0;
+    LMStepTrace step;
+    lm.trace = &step;
+    trace.clear();
     while (true) {
       if (iteration >= (size_t)prm.trk_max_iteration) break;
-      setStochasticSampling((iteration % numBatches) * prm.trk_batch_size, prm.trk_batch_size);
+      const size_t offset = (iteration % numBatches) * prm.trk_batch_size;
+      setStochasticSampling(offset, prm.trk_batch_size);
       std::vector<double> x(6, 0.0);
+      double R0[9], t0[3];
+      std::memcpy(R0, R_, sizeof(R0)); std::memcpy(t0, t_, sizeof(t0));
       if (lm.minimizeInit(x, (int)numPoints) == LM_ImproperInputParameters) return -1;
       LMStatus status = lm.minimizeOneStep(x);
+      const double head[10] = {(double)offset, (double)numPoints, (double)status, (double)lm.nfev, (double)step.rank,
+                               (double)step.nonzero_pivots, (double)step.downdate_recomputes, (double)step.trials.size(),
+                               step.fnorm, step.gnorm};
+      trace.insert(trace.end(), head, head + 10);
+      trace.insert(trace.end(), R0, R0 + 9);
+      trace.insert(trace.end(), t0, t0 + 3);
+      for (const auto& t : step.trials) {
+        trace.insert(trace.end(), t.x.begin(), t.x.end());
+        const double rec[TRACE_TRIAL - 6] = {t.fnorm1, t.actred, t.prered, t.ratio, t.par, t.delta, t.xnorm,
+                                             (double)t.accepted, (double)t.lmpar_iter};
+        trace.insert(trace.end(), rec, rec + TRACE_TRIAL - 6);
+      }
       addMotionUpdate(x.data());
       iteration++;
       nfev += lm.nfev;

@@ -326,6 +326,16 @@ OAPI int esvo_oracle_track_get_negative_ts(esvo_oracle_ctx* c, double* neg, doub
   return ESVO_OK;
 }
 
+// Trace of the last esvo_oracle_track_solve (RegProblem::trace for the layout): copies up to cap doubles, *n = its length.
+OAPI int esvo_oracle_track_trace(esvo_oracle_ctx* c, double* out, size_t cap, size_t* n) {
+  if (!c || !n) return ESVO_ERR_INVALID_ARG;
+  const auto& t = c->reg.trace;
+  *n = t.size();
+  if (t.size() > cap) return ESVO_ERR_CAPACITY;
+  if (!t.empty()) std::memcpy(out, t.data(), t.size() * sizeof(double));
+  return ESVO_OK;
+}
+
 // Pinning tap (tests/test_indep_pins.py): after esvo_oracle_track_reset, select batch 0 like the first solver iteration
 // and return RegProblemLM::operator()(x) and df(0) for it, with the inputs an independent evaluation needs:
 // pts (3 per point, ref frame), Rt = {R_ row-major (9), t_ (3)}.  fjac is row-major n x 6.  Returns the batch size.

@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 
 from esvo_b200 import capi, configs, synth
-from util import build_ts_pair, fold_replay, fold_vector, grid_vs_map, make_backends, rel, scenario
+from util import (TRACK_CASES, build_ts_pair, fold_replay, fold_vector, grid_vs_map, make_backends, rel, scenario, track_backend,
+                  track_inputs, track_params, track_trace)
 
 pytestmark = pytest.mark.gpu
 
@@ -561,55 +562,121 @@ def test_initialization_from_sgm_disparity(oracle_lib, product_lib):
     assert fin.sum() > 500 and (r < 1e-4).mean() > 0.995 and np.median(r) < 1e-7
 
 
-def _tracking_case(oracle_lib, product_lib, rig, analytical, perturb=True, seed=11):
-    s = scenario(rig)
-    o, g = make_backends(rig, oracle_lib, product_lib)
-    tl, _ = build_ts_pair(o, s)
-    rng = np.random.default_rng(seed)
-    # reference cloud: scene points visible from the current view, world frame, float32 like pcl::PointXYZ
-    pts = s["scene_points"]
-    Tw = s["T_world_left"]
-    pc = (pts - Tw[:3, 3]) @ Tw[:3, :3]
-    vis = pc[:, 2] > 0.1
-    sel = rng.choice(np.nonzero(vis)[0], size=min(6000, vis.sum()), replace=False)
-    cloud = pts[sel].astype(np.float32)
-    T_ref = Tw.copy()
-    T_prior = Tw.copy()
-    if perturb:
-        T_prior[:3, 3] += np.array([0.004, -0.003, 0.002]) * (1 if rig == "hkust" else 20)
+def _track_run(c, oracle_lib, product_lib, max_iteration=None):
+    """Case c of util.TRACK_CASES on the oracle and the device, identical inputs: [(pose, stats, permuted cloud, backend)]."""
+    if max_iteration is not None:
+        c = dict(c, it=max_iteration)
+    tl, cloud, T_ref, T_prior = track_inputs(c, oracle_lib)
     res = []
-    for be in (o, g):
-        c = cloud.copy()
+    for lib in (oracle_lib, product_lib):
+        be = track_backend(c, lib, product_lib)
+        cl = cloud.copy()
         be.track_srand(1)
-        rc = be.track_reset(c, T_ref, T_prior, tl)
-        assert rc == 0
-        T, st = be.track_solve(analytical)
-        res.append((T, st, c))
-    return s, o, g, res
+        assert be.track_reset(cl, T_ref, T_prior, tl) == 0
+        T, st = be.track_solve(c["an"])
+        res.append((T, st, cl, be))
+    return res
 
 
-@pytest.mark.parametrize("rig", ["hkust", "dsec"])
-def test_tracking_negative_ts_and_sampling_bit_exact(oracle_lib, product_lib, rig):
-    s, o, g, res = _tracking_case(oracle_lib, product_lib, rig, True)
-    no, ng = o.track_get_negative_ts(), g.track_get_negative_ts()
-    for a, b in zip(no, ng):
-        assert np.array_equal(a, b)
-    assert np.array_equal(res[0][2], res[1][2]), "rand()-driven partial shuffle differs"
+# Pose bars (max abs over R and t / |t|), measured on one H100: analytic cases <= 7e-14, numerical <= 4.1e-7 (bar 1e-4).
+# The one exception is the B = 6 line cloud, built so that two pairs of Jacobian columns are parallel to 1e-5 (smallest /
+# largest singular value 1e-7): the device's reduction order is amplified by that condition number, 7.5e-7 after 20
+# iterations with identical nfev / n_iter (DESIGN.md section 9).
+TRACK_POSE_BAR = {True: 1e-8, False: 1e-4}
+ILL_CONDITIONED_BAR = 1e-5
+# The shipped hkust / dsec configurations: the solve must bring the translation from the prior's offset closer to the scene's
+# true pose (measured: 5.4 -> 3.3 / 3.0 mm on hkust, 108 -> 24 / 18 mm on dsec, analytic / numerical).
+TRACK_MOVES_TOWARDS_TRUTH = ("hkust-B500-huber50-k5-trans-an", "hkust-B500-huber50-k5-trans-num", "dsec-B300-huber50-k5-trans-an",
+                             "dsec-B300-huber50-k5-trans-num")
 
 
-@pytest.mark.parametrize("rig,analytical", [("hkust", True), ("dsec", True), ("hkust", False)])
-def test_tracking_pose_parity(oracle_lib, product_lib, rig, analytical):
-    s, o, g, res = _tracking_case(oracle_lib, product_lib, rig, analytical)
-    (To, so, _), (Tg, sg, _) = res
-    print(rig, analytical, so, sg, "\n", To, "\n", Tg)
-    assert so["n_iter"] == sg["n_iter"] and so["n_points"] == sg["n_points"] and so["nfev"] == sg["nfev"]
-    assert np.abs(To[:3, :3] - Tg[:3, :3]).max() < 1e-4
+def _pose_bar(c):
+    return ILL_CONDITIONED_BAR if c["cloud"] == "line" else TRACK_POSE_BAR[c["an"]]
+
+
+def _pose_dev(To, Tg):
     tn = max(np.linalg.norm(To[:3, 3]), 1e-3)
-    assert np.linalg.norm(To[:3, 3] - Tg[:3, 3]) / tn < 1e-4
-    # and the tracker actually moved towards the true pose
-    Tw = s["T_world_left"]
-    if analytical:   # solve_numerical performs a single LM step (RegProblemSolverLM.cpp:137)
-        assert np.linalg.norm(Tg[:3, 3] - Tw[:3, 3]) < np.linalg.norm(np.array([0.004, -0.003, 0.002]) * (1 if rig == "hkust" else 20))
+    return max(np.abs(To[:3, :3] - Tg[:3, :3]).max(), np.linalg.norm(To[:3, 3] - Tg[:3, 3]) / tn)
+
+
+@pytest.mark.parametrize("cid", list(TRACK_CASES))
+def test_tracking_negative_ts_and_sampling_bit_exact(oracle_lib, product_lib, cid):
+    c = TRACK_CASES[cid]
+    (_, _, co, o), (_, _, cg, g) = _track_run(c, oracle_lib, product_lib, max_iteration=1)
+    for a, b in zip(o.track_get_negative_ts(), g.track_get_negative_ts()):
+        assert np.array_equal(a, b)
+    assert np.array_equal(co, cg), "rand()-driven partial shuffle differs"
+
+
+@pytest.mark.parametrize("cid", list(TRACK_CASES))
+def test_tracking_pose_parity(oracle_lib, product_lib, cid):
+    """The whole RegProblemSolverLM solve of every case, device against oracle: n_points, nfev, n_iter exactly, the pose within
+    TRACK_POSE_BAR.  Where the oracle trace shows a rejected trial, also after each k = 1 .. MAX_ITERATION on fresh contexts
+    (MAX_ITERATION = k), so that equal totals cannot hide different trial sequences."""
+    c = TRACK_CASES[cid]
+    (To, so, co, o), (Tg, sg, cg, _) = _track_run(c, oracle_lib, product_lib)
+    dev = _pose_dev(To, Tg)
+    print(cid, so, sg, "pose deviation %.2e" % dev)
+    assert so == sg
+    assert np.array_equal(co, cg)
+    assert dev < _pose_bar(c), dev
+    tr = track_trace(o)
+    if c["img"] == "const" or c["cloud"] == "off":
+        # J == 0: status 4 at every iteration with x = 0.  addMotionUpdate(0) still passes R_ through the polar factor, which
+        # moves it by rounding (6.7e-16 on one H100, differently on the two sides), so the pose is the prior to 1e-15, not bit for bit
+        assert all(it["status"] == 4 for it in tr) and so["nfev"] == so["n_iter"] * (1 if c["an"] else 8)
+        T_prior = track_inputs(c, oracle_lib)[3]
+        assert dev < 1e-14 and np.abs(Tg - T_prior).max() < 1e-14 and np.abs(To - T_prior).max() < 1e-14
+    if cid in TRACK_MOVES_TOWARDS_TRUTH:   # parity cannot see both sides standing still (or walking away) together
+        Tw = scenario(c["rig"])["T_world_left"]
+        T_prior = track_inputs(c, oracle_lib)[3]
+        assert np.linalg.norm(Tg[:3, 3] - Tw[:3, 3]) < 0.7 * np.linalg.norm(T_prior[:3, 3] - Tw[:3, 3])
+    if any(not q["accepted"] for it in tr for q in it["trials"]):
+        for k in range(1, c["it"] + 1):
+            (To, so, _, ok), (Tg, sg, _, _) = _track_run(c, oracle_lib, product_lib, max_iteration=k)
+            assert so == sg, (k, so, sg)
+            assert _pose_dev(To, Tg) < _pose_bar(c), (k, _pose_dev(To, Tg))
+
+
+def test_tracking_device_ts_path_and_repeated_resets(oracle_lib, product_lib):
+    """ts_left = NULL after a device ts_build gives the host-image result; two resets in a row without re-seeding keep the
+    rand() streams (and so the shuffles and poses) equal on both sides."""
+    c = TRACK_CASES["hkust-B500-huber50-k5-trans-an"]
+    s = scenario("hkust")
+    tl, cloud, T_ref, T_prior = track_inputs(c, oracle_lib)
+    g = track_backend(c, product_lib, product_lib)
+    tl_dev, _ = build_ts_pair(g, s)
+    res = []
+    for ts in (None, tl_dev):
+        cl = cloud.copy()
+        g.track_srand(1)
+        assert g.track_reset(cl, T_ref, T_prior, ts) == 0
+        res.append((g.track_solve(True), cl))
+    assert np.array_equal(res[0][1], res[1][1]) and np.array_equal(res[0][0][0], res[1][0][0]) and res[0][0][1] == res[1][0][1]
+    o = track_backend(c, oracle_lib, product_lib)
+    o.track_srand(1); g.track_srand(1)
+    for rep in range(2):
+        out = []
+        for be in (o, g):
+            cl = cloud.copy()
+            assert be.track_reset(cl, T_ref, T_prior, tl) == 0
+            out.append((be.track_solve(True), cl))
+        assert np.array_equal(out[0][1], out[1][1]), rep
+        assert out[0][0][1] == out[1][0][1] and _pose_dev(out[0][0][0], out[1][0][0]) < 1e-8, rep
+
+
+@pytest.mark.parametrize("kw", [dict(trk_batch_size=5), dict(trk_batch_size=1025), dict(trk_kernel_size=7)], ids=str)
+def test_tracking_refuses_unsupported_parameters(oracle_lib, product_lib, kw):
+    c = TRACK_CASES["hkust-B500-huber50-k5-trans-an"]
+    tl, cloud, T_ref, T_prior = track_inputs(c, oracle_lib)
+    l, r = configs.rig_calibs("hkust")
+    p = track_params(c, product_lib)
+    for k, v in kw.items():
+        setattr(p, k, v)
+    g = capi.Backend(product_lib, l, r, p)
+    with pytest.raises(capi.EsvoError) as e:
+        g.track_reset(cloud, T_ref, T_prior, tl)
+    assert e.value.code == -6
 
 
 def test_tracking_too_few_points(oracle_lib, product_lib):
