@@ -283,6 +283,9 @@ ESVO_API esvo_ctx* esvo_create(int device, const esvo_calib* left, const esvo_ca
   if (p->patch_size_x * p->patch_size_y > kMaxPatch || p->patch_size_x < 1 || p->patch_size_y < 1 ||
       !(p->patch_size_x & 1) || !(p->patch_size_y & 1))
     return fail(ESVO_ERR_UNSUPPORTED);
+  // A negative regularisation radius is an empty neighbourhood loop in DepthRegularization::apply, but the warp form's
+  // (2r+1)^2 window would read pixel (row+1, col+1): refused rather than given a second meaning.
+  if (p->reg_radius < 0) return fail(ESVO_ERR_UNSUPPORTED);
   // The closed-form cam2World / propagation (lm.cu, fuse.cu) assume a canonical rectified projection
   // P = [fx 0 cx tx; 0 fy cy ty; 0 0 1 0] (every shipped calibration); the reference's 4x4 inverse is more general.
   for (const esvo_calib* cal : {left, right})

@@ -290,3 +290,329 @@ def track_trace(o):
                                      xnorm=t[12], accepted=bool(t[13]), lmpar_iter=int(t[14])))
         out.append(it)
     return out
+
+
+# ---- map side (fusion, clean, regularisation): one case table for the CPU pin (tests/test_map_pins.py) and the device
+# parity (tests/test_gpu_map_parity.py).  Every case runs on the hkust rig (346 x 260); a case names only what it changes.
+# norm: tdist | l2 | zncc (the map runs zncc through the Student-t path).  gen: the round-1 vector (map_round1).  pose:
+# identity (J = 1, every propagated value exactly representable) | moved (a frame pose 3 deg / 2 cm away from the world
+# and per-point observation poses a few degrees and centimetres from it).  r2: the second round, fused without a reset
+# into the oracle's round-1 map (map_round2): thr (each decision of the case analysis placed on its threshold and one ulp
+# either side) | regmap (after esvo_map_regularize: fusing into rho = -1 elements).
+MAP_DEFAULT = dict(norm="tdist", radius=0, gen="lists", pose="identity", r2=None)
+MAP_NORMS = {"tdist": capi.LSNORM_TDIST, "l2": capi.LSNORM_L2, "zncc": capi.LSNORM_ZNCC}
+
+
+def _mc(**kw):
+    c = dict(MAP_DEFAULT, **kw)
+    tag = [c["norm"], "r%d" % c["radius"], c["gen"]]
+    if c["pose"] != "identity":
+        tag.append(c["pose"])
+    if c["r2"]:
+        tag.append("then-" + c["r2"])
+    c["id"] = "-".join(tag)
+    return c
+
+
+MAP_CASES = [
+    _mc(), _mc(radius=1), _mc(norm="l2"), _mc(norm="l2", radius=1), _mc(norm="zncc"),
+    _mc(pose="moved"), _mc(norm="l2", pose="moved", radius=1), _mc(norm="zncc", pose="moved", radius=1),
+    _mc(gen="edge"), _mc(gen="edge", radius=1), _mc(norm="l2", gen="edge"), _mc(norm="l2", gen="edge", radius=1),
+    _mc(gen="guards"), _mc(gen="guards", radius=1),
+    _mc(norm="l2", gen="l2floor"), _mc(norm="l2", gen="l2floor", radius=1),
+    _mc(gen="bulk"), _mc(gen="bulk", radius=1, pose="moved"),
+    _mc(gen="thr", r2="thr"), _mc(norm="l2", gen="thr", r2="thr"), _mc(gen="thr", r2="regmap"), _mc(norm="l2", gen="thr", r2="regmap"),
+]
+assert len({c["id"] for c in MAP_CASES}) == len(MAP_CASES)
+MAP_CASES = {c["id"]: c for c in MAP_CASES}
+
+
+def map_params(c, lib):
+    p = configs.params_for("hkust", lib)
+    p.lsnorm = MAP_NORMS[c["norm"]]
+    p.fusion_radius = c["radius"]
+    return p
+
+
+def map_backends(c, oracle_lib, product_lib):
+    return make_backends("hkust", oracle_lib, product_lib, tweak=lambda p: setattr(p, "lsnorm", MAP_NORMS[c["norm"]]))
+
+
+def _nx(v, k):
+    """v moved by k ulps."""
+    for _ in range(abs(k)):
+        v = float(np.nextafter(v, np.inf if k > 0 else -np.inf))
+    return v
+
+
+def depth_for(rho):
+    """A depth z with 1.0 / z == rho exactly (None if no double within 64 ulps of 1 / rho has it)."""
+    z0 = 1.0 / rho
+    for k in range(65):
+        for z in (_nx(z0, k), _nx(z0, -k)):
+            if 1.0 / z == rho:
+                return z
+    return None
+
+
+def map_point(Pl, u, v, rho, s2=0.0, nu=4.0, var=None, res=1.0, age=0, exact=True):
+    """One DepthPoint (identity observation pose) that projects to pixel coordinates (u, v) of the left camera with inverse
+    depth rho; exact=True picks its depth so that the propagation's 1 / z gives rho to the bit.  var defaults to
+    nu / (nu - 2) * s2 (the Student-t variance; only the l2 propagation reads it)."""
+    fx, cx, fy, cy = Pl[0][0], Pl[0][2], Pl[1][1], Pl[1][2]
+    z = depth_for(rho) if exact else 1.0 / rho
+    assert z is not None, rho
+    q = np.zeros(1, capi.DEPTH_POINT_DTYPE)[0]
+    q["p_cam"] = [(u - cx) / fx * z, (v - cy) / fy * z, z]
+    q["row"], q["col"], q["x"], q["inv_depth"] = int(np.floor(v)), int(np.floor(u)), (u, v), rho
+    q["scale2"], q["nu"] = s2, nu
+    with np.errstate(all="ignore"):
+        q["variance"] = var if var is not None else np.float64(nu) / (np.float64(nu) - 2) * np.float64(s2)
+    q["residual"], q["age"] = res, age
+    q["T_world_cam"] = np.eye(4).ravel()
+    return q
+
+
+def stack_points(qs):
+    out = np.zeros(len(qs), capi.DEPTH_POINT_DTYPE)
+    for i, q in enumerate(qs):
+        out[i] = q
+    return out
+
+
+def _moved(pts, Pl, seed):
+    """Re-express a vector built for identity poses under a frame pose T_wf 3 deg / 2 cm from the world: every point gets an
+    observation pose T_wf * D (D: 1-4 deg, 0.5-2 cm) and the p_cam that puts it where it was in the frame."""
+    rng = np.random.default_rng(seed)
+    Tf = np.eye(4); Tf[:3, :3] = _rot(1, 3.0) @ _rot(0, -1.5); Tf[:3, 3] = [0.02, -0.01, 0.015]
+    out = pts.copy()
+    for q in out:
+        D = np.eye(4); D[:3, :3] = _rot(int(rng.integers(0, 3)), rng.uniform(1, 4)); D[:3, 3] = rng.uniform(-0.02, 0.02, 3)
+        Twc = Tf @ D
+        p_f = np.append(q["p_cam"], 1.0)
+        q["p_cam"] = (np.linalg.inv(D) @ p_f)[:3]
+        q["T_world_cam"] = Twc.ravel()
+    return out, Tf
+
+
+def _edge_points(Pl, W, H):
+    """Projections whose splat leaves the image, x just below 0, a NaN re-projection, points behind the camera that project
+    into the image (elements with rho < -1e-6) and, later in the vector, compatible contributions into them (the "new point"
+    branch), each with a second contribution so that the fusion runs there too."""
+    qs = []
+    for (u, v) in ((W - 1e-9, 100.5), (W - 0.5, 37.25), (170.5, H - 1e-9), (60.3, H - 0.5), (W - 1e-7, H - 1e-7), (0.0, 0.0),
+                   (0.25, 120.5), (200.5, 0.0)):
+        qs += [map_point(Pl, u, v, 0.8, s2=2e-4, nu=2.1897, res=5.0), map_point(Pl, u, v, 0.81, s2=1e-4, nu=2.1897, res=4.0)]
+    qs.append(map_point(Pl, -1e-9, 50.5, 0.7, s2=1e-4, exact=False))        # x just below 0: outside
+    qs.append(map_point(Pl, 50.5, -1e-9, 0.7, s2=1e-4, exact=False))
+    nan = map_point(Pl, 80.5, 80.5, 0.7, s2=1e-4); nan["p_cam"] = 0.0       # h = (0, 0, 0): 0 / 0 re-projection
+    qs.append(nan)
+    for i, (u, v) in enumerate(((120.5, 60.5), (240.5, 180.5), (30.5, 200.5), (W - 0.5, H - 0.5))):
+        qs.append(map_point(Pl, u, v, -0.5 - 0.25 * i, s2=1e-4, res=3.0))      # behind the camera, lands in the image
+        qs.append(map_point(Pl, u, v, 0.6, s2=2.0, nu=2.1897, res=9.0))        # 2 sigma > |0.6 - rho|: the "new point" branch
+        qs.append(map_point(Pl, u, v, 0.61, s2=1e-3, nu=2.1897, res=2.0))      # then an ordinary update of the new point
+    for i, rho in enumerate((_nx(-1e-6, -1), -1e-6, _nx(-1e-6, 1))):              # the validity threshold and its neighbours
+        qs.append(map_point(Pl, 280.5 + 20 * i, 200.5, rho, s2=1e-4, res=3.0))
+    qs.append(map_point(Pl, 140.5, 140.5, -1.0, s2=1e-4, res=3.0))              # rho = -1 exactly, then far contributions
+    qs.append(map_point(Pl, 140.5, 140.5, 0.7, s2=1e-6, res=1.0))               # not compatible: case 2.2 against rho = -1
+    return stack_points(qs)
+
+
+def _guard_points(Pl):
+    """Pairs (map element, then one update) on separate pixels that take each arm of the fast path's guards: S below 1e-200
+    and above 1e200, nu_u = 2 exactly (var = +inf), just above 2, below 2 (a negative variance: NaN sigma and a NaN
+    compatibility test), >= 1e15, denormal scale, and updates whose variance leaves (1e-200, 1e200) (sqrt vs sqrt_nr)."""
+    pairs = [
+        ((0.5, 4e-201, 3.0), (0.5000001, 5e-201, 3.0)),      # S < 1e-200
+        ((0.5, 1e-200, 3.0), (0.5000001, 2e-200, 3.0)),      # S just above 1e-200, variance below 1e-200 after the update
+        ((0.5, 6e199, 3.0), (0.5000001, 6e199, 3.0)),        # S > 1e200
+        ((0.5, 4e199, 3.0), (0.5, 4e199, 3.0)),              # S < 1e200
+        ((1e101, 4e199, 2.05), (1.09e101, 4e199, 2.05)),     # fast path, variance above 1e200 after the update
+        ((0.5, 1e-3, 2.0), (0.52, 1e-3, 2.0)),               # nu_u = 2: var = +inf, sigma = inf
+        ((0.5, 1e-3, 2.0 + 2e-15), (0.52, 1e-3, 5.0)),       # just above 2
+        ((0.5, 1e-3, 4.0), (0.52, 1e-3, 0.5)),               # nu_u = 0.5: after the update nu = 1.5 -> var < 0 -> NaN sigma
+        ((0.5, 1e-3, 4.0), (0.51, 1e-3, 1.5)),               # the propagated point's own var < 0 (NaN 2 sigma)
+        ((0.5, 1e-3, 1e15), (0.51, 1e-3, 2e15)),             # nu_u >= 1e15
+        ((0.5, 1e-3, 3e14), (0.51, 1e-3, 4e14)),             # just below
+        ((0.5, 1e-310, 3.0), (0.5, 1e-3, 3.0)),              # denormal scale of the map point (S normal)
+        ((0.5, 1e-3, 3.0), (0.5000001, 3e-312, 3.0)),        # denormal scale of the propagated point
+        ((0.5, 1e-310, 3.0), (0.5, 1e-309, 3.0)),            # both denormal (S < 1e-200)
+        ((0.5, 2e-190, 3.0), (0.5000001, 3e-190, 3.0)),      # s2 * s2 underflows to a denormal in the numerator
+        ((1e-310, 1e-3, 3.0), (2e-310, 1e-3, 3.0)),          # denormal inverse depths
+    ]
+    qs, pts_next = [], []
+    for i, ((r0, s0, n0), (r1, s1, n1)) in enumerate(pairs):
+        u, v = 20.5 + 25 * (i % 12), 20.5 + 40 * (i // 12)
+        qs.append(map_point(Pl, u, v, r0, s2=s0, nu=n0, res=2.0, exact=False))
+        pts_next.append(map_point(Pl, u, v, r1, s2=s1, nu=n1, res=1.0, exact=False))
+        pts_next.append(map_point(Pl, u, v, r1, s2=s1 * 1.5, nu=n1 + 1.0, res=0.5, exact=False))   # one more update on top
+    return stack_points(qs + pts_next)
+
+
+def _l2floor_points(Pl):
+    """l2: variances below 1e-6 on create (the propagation's floor), fuse (the update's floor) and replace."""
+    qs = []
+    for i, (v0, v1, r1) in enumerate(((1e-7, 2e-7, 0.5), (1.5e-6, 1.5e-6, 0.5), (1e-6, 1e-6, 0.5), (4e-6, 1e-8, 0.5 + 0.01),
+                                      (3e-6, 5e-7, 0.6), (2e-6, 1e-12, 0.4))):
+        u, v = 30.5 + 40 * i, 60.5
+        qs.append(map_point(Pl, u, v, 0.5, var=v0, res=3.0))
+        qs.append(map_point(Pl, u, v, r1, var=v1, res=1.0))
+    return stack_points(qs)
+
+
+def _bulk_points(Pl, seed=3):
+    """24 contributions on each of 200 pixels, all in one inverse-depth cluster: thousands of Student-t updates through the
+    fast path (rcp_nr / div_nr / sqrt_nr), compared bit for bit."""
+    rng = np.random.default_rng(seed)
+    qs = []
+    for i in range(200):
+        row, col = 12 + 24 * (i // 25), 12 + 13 * (i % 25)
+        for _ in range(24):
+            rho = 0.7 * (1 + 0.01 * rng.standard_normal())
+            s2 = (10 ** rng.uniform(-2.5, -1.0)) ** 2
+            qs.append(map_point(Pl, col + rng.uniform(0.1, 0.9), row + rng.uniform(0.1, 0.9), rho, s2=s2, nu=2.1897,
+                                var=s2 * 2.1897 / 0.1897, res=rng.uniform(1, 50), age=int(rng.integers(0, 3)), exact=False))
+    pts = stack_points(qs)
+    return pts[rng.permutation(pts.size)]
+
+
+THR_RHO = 0.5625            # 9/16; with nu = 4 the Student-t variance 2 * s2 and 2 sigma are exact powers of two
+THR_S2 = 2.0 ** -15         # var = 2^-14, 2 sigma = 2^-6
+THR_TINY_S2 = 2.0 ** -41    # 2 sigma = 2^-19
+
+
+def _thr_base(Pl, norm):
+    """Round 1 of the threshold cases: one element block per target (a 2 x 2 splat of one point), columns of 11 px."""
+    qs = []
+    for i, kind in enumerate(THR_KINDS):
+        u, v = 15.5 + 11 * (i % 30), 30.5 + 30 * (i // 30)
+        s2 = THR_TINY_S2 if kind[0] == "prop2s" else THR_S2
+        qs.append(map_point(Pl, u, v, THR_RHO, s2=s2, nu=4.0, var=2 * s2, res=2.0, age=1))
+    return stack_points(qs)
+
+
+# (decision, offset in ulps of the placed quantity): the round-2 contribution of each target pixel
+THR_KINDS = [(k, o) for k in ("map2s", "prop2s", "occl", "chi") for o in (-1, 0, 1)] + \
+            [("tie", o) for o in ("eq", "var", "res", "both")]
+
+
+def _thr_round2(m, Pl, norm):
+    """Round 2 of the threshold cases, from the round-1 map m (the oracle's): per target, one contribution placed on the
+    threshold of one decision (or one ulp off it), in f64 computed in the reference's order."""
+    qs = []
+    cell = {(int(e["row"]), int(e["col"])): e for e in m}
+    for i, (kind, off) in enumerate(THR_KINDS):
+        u, v = 15.5 + 11 * (i % 30), 30.5 + 30 * (i // 30)
+        e = cell[(int(np.floor(v)), int(np.floor(u)))]
+        rho0, var0 = float(e["inv_depth"]), float(e["variance"])
+        sdm = 2 * np.sqrt(var0)
+        if kind == "map2s":       # |prho - rho| == 2 sigma of the map point (+-1 ulp); the propagated point's own 2 sigma tiny
+            rho = _nx(rho0 + sdm, off)
+            assert off != 0 or abs(rho - rho0) == sdm
+            qs.append(map_point(Pl, u, v, rho, s2=THR_TINY_S2, var=2 * THR_TINY_S2, res=3.0))
+        elif kind == "prop2s":    # |prho - rho| == 2 sigma of the propagated point; the map point's tiny
+            sd2 = 2 * np.sqrt(2 * THR_S2)
+            rho = _nx(rho0 - sd2, -off)
+            assert off != 0 or abs(rho - rho0) == sd2
+            qs.append(map_point(Pl, u, v, rho, s2=THR_S2, var=2 * THR_S2, res=3.0))
+        elif kind == "occl":      # rho - 2 sigma == prho (+-1 ulp): not compatible at and below, compatible above
+            rho = _nx(rho0 - sdm, off)
+            assert off != 0 or rho0 - sdm == rho
+            qs.append(map_point(Pl, u, v, rho, s2=THR_S2, var=var0 if norm == "l2" else 2 * THR_S2, res=1.0))
+        elif kind == "chi":       # d2 / pvar + d2 / var on either side of 5.99 (pvar = var), searched over the depths
+            def chi(z):
+                d2 = (1.0 / z - rho0) * (1.0 / z - rho0)
+                return d2 / var0 + d2 / var0
+            z = 1.0 / (rho0 + np.sqrt(5.99 * var0 / 2))      # a larger depth: a smaller prho - rho0 and chi
+            while chi(z) < 5.99:
+                z = _nx(z, -1)
+            while chi(_nx(z, 1)) >= 5.99:
+                z = _nx(z, 1)
+            # z: the last depth with chi >= 5.99; off -1 -> the next one (chi < 5.99), +1 -> the one before (chi above)
+            rho = 1.0 / _nx(z, -off)
+            qs.append(map_point(Pl, u, v, rho, s2=THR_S2, var=var0, res=3.0))
+        else:                     # replace test on ties: pvar == var and / or pres == res (not compatible, not occluded)
+            rho = rho0 + 10 * sdm
+            s2 = THR_S2 if off in ("eq", "res") else _nx(THR_S2, -1)
+            res = float(e["residual"]) if off in ("eq", "var") else _nx(float(e["residual"]), -1)
+            var = 2 * s2
+            qs.append(map_point(Pl, u, v, rho, s2=s2, var=var, res=res))
+    return stack_points(qs)
+
+
+def _reg_round2(m, Pl, norm):
+    """After esvo_map_regularize rejected the isolated round-1 elements (rho = -1): contributions whose 2 sigma reaches -1
+    (the "new point" branch) and narrow ones (case 2.2 against rho = -1)."""
+    qs = []
+    for k, e in enumerate(m):
+        if k % 4:
+            continue
+        u, v = float(e["col"]) + 0.5, float(e["row"]) + 0.5
+        if (k // 4) % 2 == 0:
+            qs.append(map_point(Pl, u, v, 0.6, s2=1.0, nu=4.0, var=4.0, res=1.0))
+        else:
+            qs.append(map_point(Pl, u, v, 0.6, s2=1e-4, nu=4.0, var=1e-4, res=1.0))
+    return stack_points(qs)
+
+
+def map_round1(c, Pl, W=346, H=260):
+    """(points, T_world_frame) of the case's first round (fused with reset_map = 1)."""
+    gen = c["gen"]
+    if gen == "lists":
+        pts, _ = fold_vector(Pl, lengths=(1, 2, 3, 33, 65, 70, 193, 200), seed=7)
+    elif gen == "edge":
+        pts = _edge_points(Pl, W, H)
+    elif gen == "guards":
+        pts = _guard_points(Pl)
+    elif gen == "l2floor":
+        pts = _l2floor_points(Pl)
+    elif gen == "bulk":
+        pts = _bulk_points(Pl)
+    else:
+        pts = _thr_base(Pl, c["norm"])
+    if c["norm"] == "l2" and gen in ("lists", "bulk"):
+        pts["variance"] = pts["scale2"] * 2.0
+    T = np.eye(4)
+    if c["pose"] == "moved":
+        pts, T = _moved(pts, Pl, seed=5)
+    return pts, T
+
+
+def map_round2(c, m, Pl):
+    """The second-round points of case c (fused with reset_map = 0), built from the round-1 map m; None for one-round cases."""
+    if c["r2"] == "thr":
+        return _thr_round2(m, Pl, c["norm"])
+    if c["r2"] == "regmap":
+        return _reg_round2(m, Pl, c["norm"])
+    return None
+
+
+def map_vec(pts):
+    """A point vector as the dicts tests/indep_fusion.py reads."""
+    return [dict(p_cam=q["p_cam"], s2=float(q["scale2"]), nu=float(q["nu"]), var=float(q["variance"]), res=float(q["residual"]),
+                 age=int(q["age"]), T_world_cam=q["T_world_cam"]) for q in pts]
+
+
+MAP_F64 = ("inv_depth", "scale2", "nu", "variance", "residual", "x")
+
+
+def bits_equal(a, b):
+    """Element-wise: the same f64 bits, or both NaN (x86 and the GPU produce different default NaN payloads)."""
+    a = np.ascontiguousarray(a, np.float64); b = np.ascontiguousarray(b, np.float64)
+    return (a.view(np.uint64) == b.view(np.uint64)) | (np.isnan(a) & np.isnan(b))
+
+
+def maps_bit_identical(mo, mg, tag, p_cam_rtol=1e-12):
+    """Two downloaded maps: size, element order, rows / cols, ages exact; every f64 field but p_cam bit-identical; p_cam
+    within p_cam_rtol (closed-form cam2World on the device, DESIGN.md deviation 3)."""
+    assert mo.size == mg.size, (tag, mo.size, mg.size)
+    assert np.array_equal(mo["row"], mg["row"]) and np.array_equal(mo["col"], mg["col"]), tag + ": element order"
+    assert np.array_equal(mo["age"], mg["age"]), tag + ": ages"
+    for f in MAP_F64:
+        eq = bits_equal(mo[f], mg[f])
+        assert eq.all(), (tag, f, int((~eq).sum()), np.nonzero(~eq.reshape(len(mo), -1).all(axis=1))[0][:5],
+                          mo[f][~eq][:3], mg[f][~eq][:3])
+    pc_o, pc_g = mo["p_cam"], mg["p_cam"]
+    fin = np.isfinite(pc_o)
+    assert np.array_equal(fin, np.isfinite(pc_g)), tag + ": p_cam finiteness"
+    assert np.allclose(pc_g[fin], pc_o[fin], rtol=p_cam_rtol, atol=1e-300), (tag, "p_cam", np.abs(pc_g[fin] - pc_o[fin]).max())
