@@ -13,8 +13,6 @@
 // 105 px x 4 B = 420 B (SURVEY.md 8d, f32 TS convention).
 #include <cuda.h>      // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint, libcuda is not linked)
 
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace esvo {
@@ -361,11 +359,10 @@ int bm_run(Ctx* c) {
   a.ex = c->d_ex; a.ey = c->d_ey; a.et = c->d_et; a.n = (int)c->n_ev; a.lut = c->d_lut; a.mask = c->d_mask;
   a.tl = c->obs_ls; a.tr = c->obs_rs; a.pose_t = c->d_pose_t; a.n_poses = (int)c->n_poses; a.out = c->bm;
   a.counters = (unsigned long long*)c->d_counters;
-  // TMA-staged strips by default (faster than per-lane loads, identical results);
-  // ESVO_BM_TMA=0 selects the per-lane LDG kernel, which also serves step > 1, the up-down rig and very wide searches
-  static const int use_tma = getenv("ESVO_BM_TMA") ? atoi(getenv("ESVO_BM_TMA")) : 1;
+  // TMA-staged strips (faster than per-lane loads, identical results); the per-lane LDG kernel serves step > 1, the up-down
+  // rig, very wide searches and a failed tensor-map encode
   const int strip = c->dc.wx + c->dc.dmax - c->dc.dmin + 15;     // + alignment slack of the box origin
-  if (use_tma && c->dc.step == 1 && !c->dc.updown && c->dc.wy <= 8 && strip <= 112 && c->dc.dmax >= c->dc.dmin) {
+  if (c->dc.step == 1 && !c->dc.updown && c->dc.wy <= 8 && strip <= 112 && c->dc.dmax >= c->dc.dmin) {
     CUtensorMap tm;
     const int bw = strip <= 64 ? 64 : 112;
     if (make_u8_tensor_map(&tm, c->obs_rs, c->dc.W, c->dc.H, c->dc.pitch, bw, c->dc.wy)) {

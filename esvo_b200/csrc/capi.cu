@@ -53,14 +53,13 @@ int map_alloc_inputs(Ctx* c, size_t n_ev, size_t n_poses) {
   if (n_ev > c->ev_cap) {
     size_t cap = std::max<size_t>(n_ev, 1024);
     void* olds[] = {c->bm.flag, c->bm.disp, c->bm.pose_idx, c->bm.cost, c->bm.xrect,
-                    c->d_seeds, c->lm_flag, c->lm_res, c->d_pts, c->lm_dbg};
+                    c->d_seeds, c->lm_flag, c->lm_res, c->d_pts};
     for (void* p : olds) if (p) cudaFree(p);
     ESVO_CUDA_TRY(c, dmalloc(&c->bm.flag, cap)); ESVO_CUDA_TRY(c, dmalloc(&c->bm.disp, cap));
     ESVO_CUDA_TRY(c, dmalloc(&c->bm.pose_idx, cap)); ESVO_CUDA_TRY(c, dmalloc(&c->bm.cost, cap));
     ESVO_CUDA_TRY(c, dmalloc(&c->bm.xrect, 2 * cap)); ESVO_CUDA_TRY(c, dmalloc(&c->d_seeds, cap));
     ESVO_CUDA_TRY(c, dmalloc(&c->lm_flag, cap)); ESVO_CUDA_TRY(c, dmalloc(&c->lm_res, 3 * cap));
     ESVO_CUDA_TRY(c, dmalloc(&c->d_pts, cap));
-    ESVO_CUDA_TRY(c, dmalloc(&c->lm_dbg, 4 * cap));
     c->ev_cap = cap;
   }
   if (n_poses > c->pose_cap) c->pose_cap = std::max<size_t>(n_poses, 256);
@@ -100,7 +99,7 @@ int stage_inputs_packed(Ctx* c, const uint16_t* ex, const uint16_t* ey, const in
 }
 
 #define SLOT_FIELDS(X) X(obs_l) X(obs_r) X(obs_ls) X(obs_rs) X(ev_cap) X(pose_cap) X(n_ev) X(n_poses) \
-  X(d_ex) X(d_ey) X(d_et) X(d_pose_t) X(d_poses) X(d_in) X(h_in) X(in_bytes) X(ev_in) X(ev_in_valid) X(bm) X(d_seeds) X(lm_flag) X(lm_res) X(lm_dbg) X(d_pts) X(d_counters) \
+  X(d_ex) X(d_ey) X(d_et) X(d_pose_t) X(d_poses) X(d_in) X(h_in) X(in_bytes) X(ev_in) X(ev_in_valid) X(bm) X(d_seeds) X(lm_flag) X(lm_res) X(d_pts) X(d_counters) \
   X(h_counters) X(h_pin) X(map)
 void slot_save(Ctx* c) {
   SlotBufs& s = c->slots[c->cur];
@@ -214,13 +213,6 @@ ESVO_API const char* esvo_version(void) { return "esvo_b200 0.1 (sm_90a)"; }
 ESVO_API const char* esvo_last_error(esvo_ctx* c) { return c ? c->err.c_str() : "null ctx"; }
 ESVO_API void* esvo_stream(esvo_ctx* c) { return c ? (void*)c->stream : nullptr; }
 ESVO_API uint64_t esvo_launch_count(esvo_ctx* c) { return c ? c->launches : 0; }
-ESVO_API int esvo_debug_lm_timing(esvo_ctx* c, long long* out, size_t n) {
-  if (!c || !c->lm_dbg) return ESVO_ERR_STATE;
-  cudaSetDevice(c->device);
-  ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-  ESVO_CUDA_TRY(c, cudaMemcpy(out, c->lm_dbg, std::min(n, c->ev_cap) * 32, cudaMemcpyDeviceToHost));
-  return ESVO_OK;
-}
 ESVO_API int esvo_sync(esvo_ctx* c) { CHECK_CTX(c); return drain(c); }
 // Measured FP64 FMA rate of this GPU (bench.py: the denominator of the fp64 roofline): SMs*8 blocks x 256 threads, two
 // independent dependent-FMA chains per thread, CUDA-event timed on the ctx stream.  Returns TFLOP/s (2 flops per FMA).
@@ -349,7 +341,7 @@ ESVO_API void esvo_destroy(esvo_ctx* c) {
   for (int i = 0; i < kMaxSlots; ++i) {
     SlotBufs& s = c->slots[i];
     void* ps[] = {s.obs_l, s.obs_r, s.own_ls, s.own_rs, s.d_counters, s.d_in, s.bm.flag, s.bm.disp, s.bm.pose_idx, s.bm.cost, s.bm.xrect, s.d_seeds, s.lm_flag, s.lm_res,
-                  s.d_pts, s.lm_dbg};
+                  s.d_pts};
     for (void* p : ps) if (p) cudaFree(p);
     if (s.h_counters) cudaFreeHost(s.h_counters);
     if (s.h_pin) cudaFreeHost(s.h_pin);

@@ -1,7 +1,6 @@
 // esvo_b200 product code -- C ABI, part 2: culling, fusion, map and whole-frame mapping entry points.
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 
 #include "common.cuh"
@@ -113,8 +112,6 @@ static int run_mapping_frame(Ctx* c) {
   }
   ESVO_CUDA_TRY(c, cudaEventRecord(sl.ev_pts, c->stream));
   sl.ev_pts_valid = true;
-  static const int dbg_skip_fuse = getenv("ESVO_DBG_SKIP_FUSE") ? atoi(getenv("ESVO_DBG_SKIP_FUSE")) : 0;   // experiment only
-  if (dbg_skip_fuse) { ESVO_CUDA_TRY(c, cudaEventRecord(sl.ev_fuse, c->stream)); sl.ev_fuse_valid = true; c->frame_no++; return ESVO_OK; }
   pe = c->prof_begin(5);
   if ((rc = fuse_reset_map(c, c->T_world_left))) return rc;               // :268-272 fresh DepthFrame at the obs pose
   {  // size the staging area once for a full window so that steady-state frames never reallocate

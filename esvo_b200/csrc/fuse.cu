@@ -15,7 +15,6 @@
 // sequence numbers).  The map is a dense SoA over the image (the SmartGrid's element list order
 // is kept as a "first touched" sequence number per pixel).
 #include <algorithm>
-#include <cstdlib>
 
 #include "common.cuh"
 
@@ -150,7 +149,7 @@ __global__ void fuse_stage_kernel(DevConsts dc, FrameSet fs, Pose16 Tfw, int rad
 
 // ---- fold: DepthFusion::fusion (:123-190) replayed per pixel in sequence order ----
 // NAIVE = DepthFusion::naive_propagation (:232-288): same ordered replay, but nearest-wins instead of fusion.
-struct CleanArgs { int enable; double var_thr, age_thr, rmax, rmin; int fast_div, net_sort, dbg_phase; };   // dbg_phase: timing probe (scripts/fold_probe.py), 0 = off
+struct CleanArgs { int enable; double var_thr, age_thr, rmax, rmin; };
 
 // ---- fold: DepthFusion::fusion (:123-190) replayed per pixel in sequence order ----
 // The state of one map pixel while its contribution list is replayed.
@@ -164,7 +163,6 @@ struct FoldState {
   // p_cam is overwritten by every create / fuse step and never read back by the recurrence, so it is evaluated once at the
   // end from the inverse depth that set it last (pc_rho); a replacement copies the propagated p_cam.
   bool pc_pending;
-  bool fast;           // branch-free division / square root in the Student-t update (ESVO_FOLD_FASTDIV, default on)
   double pc_rho;
   double sdm;          // 2*sqrt(var) of the map point, refreshed whenever var changes
 };
@@ -232,7 +230,7 @@ __device__ __forceinline__ void fold_apply(const DevConsts& dc, const PropSoA& P
       const double nu_u = fmin(pnu, f.nu);
       const double S = f.s2 + ps2;
       const double dd = f.rho - prho;
-      if (f.fast && S > 1e-200 && S < 1e200 && nu_u > 2.0 && nu_u < 1e15) {
+      if (S > 1e-200 && S < 1e200 && nu_u > 2.0 && nu_u < 1e15) {
         // the three divisions by S share one reciprocal; every quotient gets its own remainder correction (Markstein), i.e.
         // the correctly rounded value except for rare 1-ulp cases -- same arithmetic, a third of the dependent latency
         const double xr = rcp_nr(S);
@@ -303,7 +301,6 @@ __device__ __forceinline__ void heap_sort_i32(int* ids, int cnt) {
 // pixels).  A fold warp lives as long as the longest list among its 32 pixels: in first-touch order the sum of the per-warp
 // maxima is 2.5x the sum in sorted order (13 140 vs 5 320 replay steps on the bench frame, ideal 5 230), and that warp-slot
 // time is what the fold costs the frame pipeline.  Launching the longest lists first also shortens the kernel's tail.
-constexpr int FOLD_LONG = 64;        // lists longer than this are folded by a whole warp (fuse_fold_hybrid_kernel)
 __global__ void __launch_bounds__(1024) fold_order_kernel(const int32_t* __restrict__ active, const int32_t* __restrict__ pcnt,
                                                           unsigned long long* __restrict__ scal, int32_t* __restrict__ sorted) {
   __shared__ int s_hist[256], s_base[256];
@@ -314,7 +311,7 @@ __global__ void __launch_bounds__(1024) fold_order_kernel(const int32_t* __restr
   __syncthreads();
   if (threadIdx.x == 0) {
     int run = 0;
-    for (int b = 255; b >= 0; --b) { s_base[b] = run; run += s_hist[b]; if (b == FOLD_LONG + 1) scal[6] = (unsigned long long)run; }   // lists longer than FOLD_LONG
+    for (int b = 255; b >= 0; --b) { s_base[b] = run; run += s_hist[b]; }
   }
   __syncthreads();
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
@@ -348,53 +345,22 @@ __device__ __forceinline__ void network_sort_local(int* ids, int cnt) {
 #pragma unroll
   for (int i = 0; i < N; ++i) if (i < cnt) ids[i] = v[i];
 }
-__device__ __forceinline__ void sort_ids(int* ids, int cnt, bool network) {
-  if (cnt <= 16 && !network) { for (int a = 1; a < cnt; ++a) { int v = ids[a], b = a - 1; while (b >= 0 && ids[b] > v) { ids[b + 1] = ids[b]; --b; } ids[b + 1] = v; } }
-  else if (network && cnt <= 32) network_sort_local<32>(ids, cnt);
-  else if (network && cnt <= 64) network_sort_local<64>(ids, cnt);
-  else heap_sort_i32(ids, cnt);   // O(L log L) on the local array
-}
 // Lists longer than the local array (dense scenes; the 640x480 rig with fusion radius 1): kept out of line so that its
-// registers (run heads of the k-way merge) do not count against the common path.
+// registers do not count against the common path.
 template <bool NAIVE>
 __device__ __noinline__ void fold_long_list(const DevConsts& dc, const PropSoA& P, FoldState& f, int row, int col, int h, int total,
                                             const int32_t* __restrict__ next, int32_t* sort_pool, unsigned long long* scal,
-                                            unsigned long long seq_base, const CleanArgs& clean) {
+                                            unsigned long long seq_base) {
   int* seg = sort_pool + atomicAdd(&scal[5], (unsigned long long)total);
   int k = 0;
   for (int q = h; q >= 0; q = next[q]) seg[k++] = q;
-  const int nruns = (total + 63) >> 6;
-  if (clean.net_sort >= 3 && nruns <= 32) {
-    // up to 2 048 ids: runs of 64 sorted in place by the register network, then a k-way merge driven by the replay (the
-    // cached heads of the runs are scanned per step) instead of a heap sort with two dependent global accesses per sift
-    for (int r = 0; r < nruns; ++r) network_sort_local<64>(seg + 64 * r, min(64, total - 64 * r));
-    int hpos[32], hval[32];
-    for (int r = 0; r < nruns; ++r) { hpos[r] = 64 * r; hval[r] = seg[64 * r]; }
-    auto pop = [&]() -> int {
-      int best = 0x7fffffff, which = 0;
-      for (int r = 0; r < nruns; ++r) if (hval[r] < best) { best = hval[r]; which = r; }
-      const int p = ++hpos[which];
-      hval[which] = (p < min(64 * (which + 1), total)) ? seg[p] : 0x7fffffff;
-      return best;
-    };
-    int id_cur = pop();
-    FoldRec cur = P.hot[id_cur / 9];
-    for (int a = 0; a < total; ++a) {
-      int id_nxt = id_cur;
-      FoldRec nxt = cur;
-      if (a + 1 < total) { id_nxt = pop(); nxt = P.hot[id_nxt / 9]; }
-      fold_apply<NAIVE>(dc, P, f, row, col, id_cur, cur, seq_base);
-      id_cur = id_nxt; cur = nxt;
-    }
-  } else {
-    sort_ids(seg, total, false);
-    FoldRec cur = P.hot[seg[0] / 9];
-    for (int a = 0; a < total; ++a) {
-      FoldRec nxt = cur;
-      if (a + 1 < total) nxt = P.hot[seg[a + 1] / 9];
-      fold_apply<NAIVE>(dc, P, f, row, col, seg[a], cur, seq_base);
-      cur = nxt;
-    }
+  heap_sort_i32(seg, total);
+  FoldRec cur = P.hot[seg[0] / 9];
+  for (int a = 0; a < total; ++a) {
+    FoldRec nxt = cur;
+    if (a + 1 < total) nxt = P.hot[seg[a + 1] / 9];
+    fold_apply<NAIVE>(dc, P, f, row, col, seg[a], cur, seq_base);
+    cur = nxt;
   }
 }
 template <bool NAIVE>
@@ -414,18 +380,15 @@ __global__ void fuse_fold_kernel(DevConsts dc, MapSoA M, PropSoA P, int32_t* hea
   int cnt = 0, total = 0;
   for (int q = h; q >= 0; q = next[q]) { if (cnt < CAP) ids[cnt++] = q; ++total; }
   const int row = pix / dc.W, col = pix - row * dc.W;
-  if (clean.dbg_phase == 1) { if (total == 0x7fffffff) M.rho[pix] = ids[0]; return; }          // probe: list walk only
   FoldState f;
   fold_load(M, pix, row, col, f);
-  f.fast = clean.fast_div != 0;
-  if (total <= CAP && cnt > 64 && clean.net_sort >= 2) {
+  if (total <= CAP && cnt > 64) {
     // 65..192 ids: up to three runs of 64, each sorted by the register network, merged on the fly by the replay (the head
     // of every run is compared per step) -- no heap sort in local memory (0.13 of the 0.33 ms the fusion stage takes alone)
     const int e0 = 64, e1 = min(cnt, 128), e2 = cnt;
     network_sort_local<64>(ids, 64);
     network_sort_local<64>(ids + 64, e1 - 64);
     if (cnt > 128) network_sort_local<64>(ids + 128, e2 - 128);
-    if (clean.dbg_phase == 2) { if (ids[cnt - 1] == 0x7fffffff) M.rho[pix] = ids[0]; return; }  // probe: walk + sort
     int h0 = 0, h1 = 64, h2 = 128;
     auto pop = [&]() -> int {
       int best = 0x7fffffff, which = 0;
@@ -445,8 +408,8 @@ __global__ void fuse_fold_kernel(DevConsts dc, MapSoA M, PropSoA P, int32_t* hea
       id_cur = id_nxt; cur = nxt;
     }
   } else if (total <= CAP) {
-    sort_ids(ids, cnt, clean.net_sort != 0);
-    if (clean.dbg_phase == 2) { if (ids[cnt - 1] == 0x7fffffff) M.rho[pix] = ids[0]; return; }  // probe: walk + sort
+    if (cnt <= 32) network_sort_local<32>(ids, cnt);
+    else network_sort_local<64>(ids, cnt);
     FoldRec cur = P.hot[ids[0] / 9];
     for (int a = 0; a < cnt; ++a) {              // the next record is in flight while this one is folded
       FoldRec nxt = cur;
@@ -457,201 +420,9 @@ __global__ void fuse_fold_kernel(DevConsts dc, MapSoA M, PropSoA P, int32_t* hea
   } else {
     // long list (dense scenes: several hundred contributions on one pixel): its ids go to a private segment of the sort pool
     // (the pool holds one int per contribution, so the segments of all pixels always fit), heap-sorted there, replayed as above
-    fold_long_list<NAIVE>(dc, P, f, row, col, h, total, next, sort_pool, scal, seq_base, clean);
+    fold_long_list<NAIVE>(dc, P, f, row, col, h, total, next, sort_pool, scal, seq_base);
   }
   fold_store(dc, M, pix, f, clean, cbits, seq_base, scal);
-}
-
-// Hybrid form (ESVO_FOLD_HYBRID=1, latency-critical use; NOT the default): the length-sorted active list starts with the long lists (> FOLD_LONG contributions, scal[6] of
-// them).  Those go one per WARP to the first G_long blocks: lane 0 walks the list into shared memory, the 32 lanes sort it
-// there with a bitonic network, fetch the 48-byte records 32 at a time and broadcast them step by step to a replay that runs
-// redundantly in every lane (uniform control flow; lane 0 stores).  A thread's heap sort of a long list in local memory costs
-// more than its replay, and in the 640x480 rig (fusion radius 1: lists of several hundred ids, heap-sorted in the global pool)
-// the long lists dominate the fusion stage.  All other blocks fold 32 short lists each, one per thread, with the register
-// sorting network.  Alone the fusion stage gets faster -- but in the frame pipeline a warp that replays ONE list in 32
-// redundant lanes spends 32x the issue slots of a lane that replays it next to 31 other lists.  Throughput wants the thread form.
-constexpr int FOLD_CAPL = 1024;      // ids of a long list held in shared memory; beyond that lane 0 falls back to the pool heap sort
-template <bool NAIVE>
-__global__ void __launch_bounds__(32, 16) fuse_fold_hybrid_kernel(DevConsts dc, MapSoA M, PropSoA P, int32_t* head, const int32_t* __restrict__ next,
-                                                              const int32_t* __restrict__ sorted, int32_t* pcnt, unsigned long long seq_base,
-                                                              unsigned long long* scal, uint32_t* cbits, CleanArgs clean, int32_t* sort_pool,
-                                                              int G_long) {
-  __shared__ int s_ids[FOLD_CAPL];
-  const unsigned FULLM = 0xffffffffu;
-  const int lane = threadIdx.x;
-  const int n_active = (int)scal[3], n_long = min((int)scal[6], n_active);
-  if ((int)blockIdx.x >= G_long) {
-    // ---------------- short lists: one per thread ----------------
-    const int t = n_long + ((int)blockIdx.x - G_long) * 32 + lane;
-    if (t >= n_active) return;
-    const int pix = sorted[t];
-    const int h = head[pix];
-    if (h < 0) return;               // listed twice: the first copy folded it
-    head[pix] = -1;
-    pcnt[pix] = 0;
-    constexpr int CAP = 192;
-    int ids[CAP];
-    int cnt = 0, total = 0;
-    for (int q = h; q >= 0; q = next[q]) { if (cnt < CAP) ids[cnt++] = q; ++total; }
-    const int row = pix / dc.W, col = pix - row * dc.W;
-    FoldState f;
-    fold_load(M, pix, row, col, f);
-    f.fast = clean.fast_div != 0;
-    int* seq = ids;
-    if (total > CAP) {               // cannot happen while pcnt is exact; kept as the general fallback
-      seq = sort_pool + atomicAdd(&scal[5], (unsigned long long)total);
-      int k = 0;
-      for (int q = h; q >= 0; q = next[q]) seq[k++] = q;
-      sort_ids(seq, total, false);
-    } else sort_ids(ids, cnt, true);
-    FoldRec cur = P.hot[seq[0] / 9];
-    for (int a = 0; a < total; ++a) {              // the next record is in flight while this one is folded
-      FoldRec nxt = cur;
-      if (a + 1 < total) nxt = P.hot[seq[a + 1] / 9];
-      fold_apply<NAIVE>(dc, P, f, row, col, seq[a], cur, seq_base);
-      cur = nxt;
-    }
-    fold_store(dc, M, pix, f, clean, cbits, seq_base, scal);
-    return;
-  }
-  // ---------------- long lists: one per warp ----------------
-  for (int t = blockIdx.x; t < n_long; t += G_long) {
-    const int pix = sorted[t];
-    int h = 0, total = 0;
-    int* seq = s_ids;
-    if (lane == 0) {
-      h = head[pix];
-      if (h >= 0) {
-        head[pix] = -1;
-        pcnt[pix] = 0;
-        for (int q = h; q >= 0; q = next[q]) { if (total < FOLD_CAPL) s_ids[total] = q; ++total; }   // serial list walk
-      }
-    }
-    h = __shfl_sync(FULLM, h, 0); total = __shfl_sync(FULLM, total, 0);
-    if (h < 0) continue;
-    if (total > FOLD_CAPL) {         // very long list: pool segment, heap-sorted by lane 0
-      unsigned long long base = 0;
-      if (lane == 0) {
-        base = atomicAdd(&scal[5], (unsigned long long)total);
-        int* seg = sort_pool + base;
-        int k = 0;
-        for (int q = h; q >= 0; q = next[q]) seg[k++] = q;
-        heap_sort_i32(seg, total);
-        __threadfence_block();
-      }
-      base = __shfl_sync(FULLM, base, 0);
-      seq = sort_pool + base;
-    } else {
-      int N = 64;
-      while (N < total) N <<= 1;
-      for (int i = total + lane; i < N; i += 32) s_ids[i] = 0x7fffffff;
-      __syncwarp();
-      for (int k = 2; k <= N; k <<= 1)
-        for (int j = k >> 1; j > 0; j >>= 1) {
-          for (int i = lane; i < N; i += 32) {
-            const int l = i ^ j;
-            if (l > i) {
-              const int a = s_ids[i], b = s_ids[l];
-              if ((a > b) == ((i & k) == 0)) { s_ids[i] = b; s_ids[l] = a; }
-            }
-          }
-          __syncwarp();
-        }
-    }
-    __syncwarp();
-    const int row = pix / dc.W, col = pix - row * dc.W;
-    FoldState f;
-    fold_load(M, pix, row, col, f);
-    f.fast = clean.fast_div != 0;
-    FoldRec mine;                    // record of step base + lane, fetched one chunk ahead
-    { const int e = lane < total ? lane : 0; mine = P.hot[seq[e] / 9]; }
-    for (int base = 0; base < total; base += 32) {
-      const FoldRec cur = mine;
-      if (base + 32 < total) { const int e = base + 32 + lane < total ? base + 32 + lane : base + 32; mine = P.hot[seq[e] / 9]; }
-      const int nstep = min(32, total - base);
-      for (int k = 0; k < nstep; ++k) {
-        FoldRec r;
-        r.rho = __shfl_sync(FULLM, cur.rho, k); r.s2 = __shfl_sync(FULLM, cur.s2, k); r.nu = __shfl_sync(FULLM, cur.nu, k);
-        r.var = __shfl_sync(FULLM, cur.var, k); r.res = __shfl_sync(FULLM, cur.res, k); r.sd2 = __shfl_sync(FULLM, cur.sd2, k);
-        fold_apply<NAIVE>(dc, P, f, row, col, seq[base + k], r, seq_base);
-      }
-    }
-    if (lane == 0) fold_store(dc, M, pix, f, clean, cbits, seq_base, scal);
-    __syncwarp();
-  }
-}
-
-// Warp-per-active-pixel form (ESVO_FOLD_WARP=1): lower latency alone, more warp-slot time in the pipeline.  A pixel's replay is inherently serial (every step depends on the state the previous one
-// left), so the 32 lanes cannot share ONE replay -- but they can take everything around it: the contribution ids are rank-sorted
-// by all lanes in shared memory (no local-memory heap sort), the 48-byte records of the next 32 steps are fetched by 32 lanes
-// at once (one gather instead of 32 dependent loads) and broadcast step by step; the replay itself runs redundantly in every
-// lane (uniform control flow, lane 0 stores).  With one warp per pixel there are thousands of warps to hide the list walk and
-// the division chains of each other, where the thread form has ~1.5 warps per SM.
-constexpr int FOLD_CAPW = 256;        // ids per pixel held in shared memory; longer lists take the selection walk
-// FOLD_WPB warps per block.  One-warp blocks (4 K registers) slot into the holes single LM blocks leave in a busy SM; bigger
-// blocks wait for several neighbouring LM warps to retire.
-template <bool NAIVE, int FOLD_WPB>
-__global__ void __launch_bounds__(FOLD_WPB * 32, 16 / FOLD_WPB) fuse_fold_warp_kernel(DevConsts dc, MapSoA M, PropSoA P, int32_t* head,
-                                                                        const int32_t* __restrict__ next, const int32_t* __restrict__ active, int32_t* pcnt,
-                                                                        unsigned long long seq_base, unsigned long long* scal, uint32_t* cbits,
-                                                                        CleanArgs clean) {
-  __shared__ int s_ids[FOLD_WPB][FOLD_CAPW], s_sorted[FOLD_WPB][FOLD_CAPW];
-  const unsigned FULLM = 0xffffffffu;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int nwarps = gridDim.x * FOLD_WPB;
-  const int n_active = (int)scal[3];
-  for (int t = blockIdx.x * FOLD_WPB + w; t < n_active; t += nwarps) {
-    const int pix = active[t];
-    int h = 0, total = 0;
-    if (lane == 0) {
-      h = head[pix];
-      if (h >= 0) {
-        head[pix] = -1;
-        pcnt[pix] = 0;
-        for (int q = h; q >= 0; q = next[q]) { if (total < FOLD_CAPW) s_ids[w][total] = q; ++total; }   // serial list walk
-      }
-    }
-    h = __shfl_sync(FULLM, h, 0); total = __shfl_sync(FULLM, total, 0);
-    if (h < 0) continue;             // listed twice: the first copy folded it
-    __syncwarp();
-    const int row = pix / dc.W, col = pix - row * dc.W;
-    FoldState f;
-    fold_load(M, pix, row, col, f);
-    f.fast = clean.fast_div != 0;
-    if (total <= FOLD_CAPW) {
-      // rank sort: ids are distinct, rank = number of smaller ids
-      for (int e = lane; e < total; e += 32) {
-        const int v = s_ids[w][e];
-        int rank = 0;
-        for (int k = 0; k < total; ++k) rank += s_ids[w][k] < v;
-        s_sorted[w][rank] = v;
-      }
-      __syncwarp();
-      FoldRec mine;                  // record of step base + lane, fetched one chunk ahead
-      { const int e = lane < total ? lane : 0; mine = P.hot[s_sorted[w][e] / 9]; }
-      for (int base = 0; base < total; base += 32) {
-        const FoldRec cur = mine;
-        if (base + 32 < total) { const int e = base + 32 + lane < total ? base + 32 + lane : base + 32; mine = P.hot[s_sorted[w][e] / 9]; }
-        const int nstep = min(32, total - base);
-        for (int k = 0; k < nstep; ++k) {
-          FoldRec r;
-          r.rho = __shfl_sync(FULLM, cur.rho, k); r.s2 = __shfl_sync(FULLM, cur.s2, k); r.nu = __shfl_sync(FULLM, cur.nu, k);
-          r.var = __shfl_sync(FULLM, cur.var, k); r.res = __shfl_sync(FULLM, cur.res, k); r.sd2 = __shfl_sync(FULLM, cur.sd2, k);
-          fold_apply<NAIVE>(dc, P, f, row, col, s_sorted[w][base + k], r, seq_base);
-        }
-      }
-    } else {   // very long list: repeated minimum selection over the list, every lane walks (uniform), no storage
-      int last = -1;
-      for (int a = 0; a < total; ++a) {
-        int best = 0x7fffffff;
-        for (int q = h; q >= 0; q = next[q]) if (q > last && q < best) best = q;
-        fold_apply<NAIVE>(dc, P, f, row, col, best, P.hot[best / 9], seq_base);
-        last = best;
-      }
-    }
-    if (lane == 0) fold_store(dc, M, pix, f, clean, cbits, seq_base, scal);
-    __syncwarp();
-  }
 }
 
 // ---- SmartGrid::clean (:222-243) ----
@@ -664,14 +435,10 @@ __global__ void map_clean_kernel(int npix, MapSoA M, double var_thr, double age_
 }
 
 // ---- DepthRegularization::apply ----
-// LIST: one thread per active pixel (valid while every existing pixel is in the list exactly once: one fold since the reset)
-template <bool LIST>
-__global__ void map_regularize_kernel(DevConsts dc, MapSoA M, int radius, int min_nb, int min_close, const int32_t* __restrict__ active,
-                                      const unsigned long long* __restrict__ scal) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  int pix = t;
-  if (LIST) { if ((unsigned long long)t >= scal[3]) return; pix = active[t]; }
-  else if (pix >= dc.W * dc.H) return;
+// Thread per image pixel: any map (map_regularize_warp_kernel needs every existing pixel listed, i.e. one fold since the reset)
+__global__ void map_regularize_kernel(DevConsts dc, MapSoA M, int radius, int min_nb, int min_close) {
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= dc.W * dc.H) return;
   if (!M.exists[pix]) return;
   const double rho = M.rho[pix];
   M.rho_tmp[pix] = rho;
@@ -1201,13 +968,7 @@ int fuse_window(Ctx* c, const Ctx::WinFrame* frames, int nframes, int radius) {
 int fuse_finish(Ctx* c, bool naive, const double* clean4) {
   MapState* ms = c->map;
   if (ms->staged == 0) return ESVO_OK;
-  CleanArgs ca{0, 0, 0, 0, 0, 0, 0, 0};
-  static const int dbg_phase = getenv("ESVO_DBG_FOLD_PHASE") ? atoi(getenv("ESVO_DBG_FOLD_PHASE")) : 0;
-  ca.dbg_phase = dbg_phase;
-  static const int net_sort = getenv("ESVO_FOLD_NETSORT") ? atoi(getenv("ESVO_FOLD_NETSORT")) : 2;   // 0 heap sort, 1 network <= 64, 2 + merged runs <= 192, 3 + merged runs in the pool (<= 2 048 ids; experiment)
-  ca.net_sort = net_sort;
-  static const int fast_div = getenv("ESVO_FOLD_FASTDIV") ? atoi(getenv("ESVO_FOLD_FASTDIV")) : 1;
-  ca.fast_div = fast_div;
+  CleanArgs ca{0, 0, 0, 0, 0};
   if (clean4) { ca.enable = 1; ca.var_thr = clean4[0]; ca.age_thr = clean4[1]; ca.rmax = clean4[2]; ca.rmin = clean4[3]; }
   // creator bits feed the sort-free ordered hand-off; only meaningful for the first fold after a reset
   uint32_t* cbits = nullptr;
@@ -1216,41 +977,16 @@ int fuse_finish(Ctx* c, bool naive, const double* clean4) {
     ESVO_CUDA_TRY(c, cudaMemsetAsync(ms->cbits, 0, ms->fold_words * 4, c->stream));
     cbits = ms->cbits;
   }
-  // at most one thread per image pixel can be active; the grid covers that bound, surplus blocks exit on the device count
-  // Thread-per-active-pixel is the production form: in the frame pipeline the fold's cost is warp-slot time next to the LM
-  // blocks, and a few hundred dense warps beat thousands of one-pixel warps there, although the warp form is faster alone.
-  // ESVO_FOLD_WARP=1 selects the warp form (latency-critical use).
-  static const int warp_fold = getenv("ESVO_FOLD_WARP") ? atoi(getenv("ESVO_FOLD_WARP")) : 0;
-  if (!warp_fold) {
-    const int npix = c->dc.W * c->dc.H, B = 32;
-    const int bound = (int)std::min<size_t>((size_t)npix, ms->staged * 9);
-    // pixels ordered by list length, longest first (ESVO_FOLD_SORT=0: first-touch order)
-    static const int sort_lists = getenv("ESVO_FOLD_SORT") ? atoi(getenv("ESVO_FOLD_SORT")) : 1;
-    const int32_t* order = ms->active;
-    if (sort_lists) {
-      fold_order_kernel<<<1, 1024, 0, c->stream>>>(ms->active, ms->pcnt, ms->d_scal, ms->active_sorted);
-      c->launches += 1;
-      order = ms->active_sorted;
-    }
-    static const int hybrid = getenv("ESVO_FOLD_HYBRID") ? atoi(getenv("ESVO_FOLD_HYBRID")) : 0;
-    if (sort_lists && hybrid && !ca.dbg_phase) {
-      const int G_long = c->num_sms * 4;     // warps that walk the long lists; the other blocks take 32 short lists each
-      if (naive) fuse_fold_hybrid_kernel<true><<<G_long + div_up(bound, B), B, 0, c->stream>>>(c->dc, ms->m, ms->p, ms->head, ms->next, order, ms->pcnt, ms->seq_base, ms->d_scal, cbits, ca, ms->sort_pool, G_long);
-      else fuse_fold_hybrid_kernel<false><<<G_long + div_up(bound, B), B, 0, c->stream>>>(c->dc, ms->m, ms->p, ms->head, ms->next, order, ms->pcnt, ms->seq_base, ms->d_scal, cbits, ca, ms->sort_pool, G_long);
-    } else if (naive) fuse_fold_kernel<true><<<div_up(bound, B), B, 0, c->stream>>>(c->dc, ms->m, ms->p, ms->head, ms->next, order, ms->pcnt, ms->seq_base, ms->d_scal, cbits, ca, ms->sort_pool);
-    else fuse_fold_kernel<false><<<div_up(bound, B), B, 0, c->stream>>>(c->dc, ms->m, ms->p, ms->head, ms->next, order, ms->pcnt, ms->seq_base, ms->d_scal, cbits, ca, ms->sort_pool);
-  } else {   // persistent: one-warp blocks walk the active list, one warp per pixel
-    static const int G_env = getenv("ESVO_DBG_FOLD_GRID") ? atoi(getenv("ESVO_DBG_FOLD_GRID")) : 0;
-    const int G = G_env ? G_env : c->num_sms * 16;
-    static const int wpb = getenv("ESVO_DBG_FOLD_WPB") ? atoi(getenv("ESVO_DBG_FOLD_WPB")) : 1;
-    if (wpb == 4) {
-      if (naive) fuse_fold_warp_kernel<true, 4><<<G, 128, 0, c->stream>>>(c->dc, ms->m, ms->p, ms->head, ms->next, ms->active, ms->pcnt, ms->seq_base, ms->d_scal, cbits, ca);
-      else fuse_fold_warp_kernel<false, 4><<<G, 128, 0, c->stream>>>(c->dc, ms->m, ms->p, ms->head, ms->next, ms->active, ms->pcnt, ms->seq_base, ms->d_scal, cbits, ca);
-    } else {
-      if (naive) fuse_fold_warp_kernel<true, 1><<<G, 32, 0, c->stream>>>(c->dc, ms->m, ms->p, ms->head, ms->next, ms->active, ms->pcnt, ms->seq_base, ms->d_scal, cbits, ca);
-      else fuse_fold_warp_kernel<false, 1><<<G, 32, 0, c->stream>>>(c->dc, ms->m, ms->p, ms->head, ms->next, ms->active, ms->pcnt, ms->seq_base, ms->d_scal, cbits, ca);
-    }
-  }
+  // Thread per active pixel: in the frame pipeline the fold's cost is warp-slot time next to the LM blocks, and a few hundred
+  // dense warps beat thousands of one-pixel warps there, although a warp per pixel is faster alone.
+  // At most one thread per image pixel can be active; the grid covers that bound, surplus blocks exit on the device count.
+  const int npix = c->dc.W * c->dc.H, B = 32;
+  const int bound = (int)std::min<size_t>((size_t)npix, ms->staged * 9);
+  // pixels ordered by list length, longest first
+  fold_order_kernel<<<1, 1024, 0, c->stream>>>(ms->active, ms->pcnt, ms->d_scal, ms->active_sorted);
+  c->launches += 1;
+  if (naive) fuse_fold_kernel<true><<<div_up(bound, B), B, 0, c->stream>>>(c->dc, ms->m, ms->p, ms->head, ms->next, ms->active_sorted, ms->pcnt, ms->seq_base, ms->d_scal, cbits, ca, ms->sort_pool);
+  else fuse_fold_kernel<false><<<div_up(bound, B), B, 0, c->stream>>>(c->dc, ms->m, ms->p, ms->head, ms->next, ms->active_sorted, ms->pcnt, ms->seq_base, ms->d_scal, cbits, ca, ms->sort_pool);
   c->launches += 1;
   ms->seq_base += (unsigned long long)ms->staged * 9ULL;
   ms->staged = 0;
@@ -1272,25 +1008,17 @@ int map_regularize(Ctx* c, bool count) {
   MapState* ms = c->map;
   const int npix = c->dc.W * c->dc.H, B = 32;
   if (list_ok(ms)) {
-    const int bound = npix;
-    static const int dbg_thread_form = getenv("ESVO_DBG_REG_THREAD") ? 1 : 0;     // experiment switch: the thread-per-pixel list form
-    if (dbg_thread_form)
-      map_regularize_kernel<true><<<div_up(bound, B), B, 0, c->stream>>>(c->dc, ms->m, c->prm.reg_radius, c->prm.reg_min_neighbours,
-                                                                        c->prm.reg_min_close_neighbours, ms->active, ms->d_scal);
-    else {   // persistent: small blocks (see fuse_fold_warp_kernel) walk the active list, one warp per pixel
-      static const int G_env = getenv("ESVO_DBG_REG_GRID") ? atoi(getenv("ESVO_DBG_REG_GRID")) : 0;
-      const int G = G_env ? G_env : c->num_sms * 16;
-      static const int T = getenv("ESVO_DBG_REG_THREADS") ? atoi(getenv("ESVO_DBG_REG_THREADS")) : 32;
-      map_regularize_warp_kernel<<<G, T, 0, c->stream>>>(c->dc, ms->m, c->prm.reg_radius, c->prm.reg_min_neighbours,
-                                                         c->prm.reg_min_close_neighbours, ms->active, ms->d_scal);
-    }
-    if (count) map_commit_count_list_kernel<<<div_up(bound, 256), 256, 0, c->stream>>>(ms->m, 1, ms->active, ms->d_scal);
+    // persistent: one-warp blocks walk the active list, one warp per pixel.  One-warp blocks (4 K registers) slot into the
+    // holes single LM blocks leave in a busy SM; bigger blocks wait for several neighbouring LM warps to retire.
+    map_regularize_warp_kernel<<<c->num_sms * 16, 32, 0, c->stream>>>(c->dc, ms->m, c->prm.reg_radius, c->prm.reg_min_neighbours,
+                                                                       c->prm.reg_min_close_neighbours, ms->active, ms->d_scal);
+    if (count) map_commit_count_list_kernel<<<div_up(npix, 256), 256, 0, c->stream>>>(ms->m, 1, ms->active, ms->d_scal);
     else map_regularize_commit_kernel<<<div_up(npix, 256), 256, 0, c->stream>>>(npix, ms->m);
     c->launches += 2;
     return ESVO_OK;
   }
-  map_regularize_kernel<false><<<div_up(npix, B), B, 0, c->stream>>>(c->dc, ms->m, c->prm.reg_radius, c->prm.reg_min_neighbours,
-                                                                     c->prm.reg_min_close_neighbours, ms->active, ms->d_scal);
+  map_regularize_kernel<<<div_up(npix, B), B, 0, c->stream>>>(c->dc, ms->m, c->prm.reg_radius, c->prm.reg_min_neighbours,
+                                                              c->prm.reg_min_close_neighbours);
   map_regularize_commit_kernel<<<div_up(npix, 256), 256, 0, c->stream>>>(npix, ms->m);
   c->launches += 2;
   if (count) return map_count(c);

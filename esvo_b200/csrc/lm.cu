@@ -19,9 +19,6 @@
 // refinements of the reciprocal / reciprocal square root.
 // Algorithmic bytes per residual evaluation: 2 x 16 x 8 px x 4 B = 1024 B (SURVEY.md 8d).
 #include <algorithm>
-#include <cstdlib>
-
-#include <cuda.h>      // CUtensorMap (types only)
 
 #include "common.cuh"
 
@@ -43,7 +40,6 @@ struct LmArgs {
   int32_t* flag;
   double* res;                      // 3 per seed
   unsigned long long* counters;
-  long long* dbg;                   // optional: 4 per seed {cycles, nfev, ns, start ns}
 };
 
 // PerspectiveCamera::cam2World (CameraSystem.cpp:120-139) for P = [fx 0 cx tx; 0 fy cy ty; 0 0 1 tz]:
@@ -121,8 +117,7 @@ __device__ __forceinline__ double irls_lane_sum(const double (&a)[S], double nus
 }
 
 // TD: LSnorm is known to be Tdist at compile time (every shipped cfg) -- sheds the l2 / zncc code and registers.
-// IRLS: 0 = one reciprocal per pixel, 1 = one reciprocal per group of four pixels.
-template <int S, bool TD, int IRLS>
+template <int S, bool TD>
 __device__ __forceinline__ void depth_residual_half(const DevConsts& dc, const SeedGeom& g, const uint8_t* __restrict__ tl,
                                                     const uint8_t* __restrict__ tr, double rho, const int (&off)[S], unsigned vmask,
                                                     double (&fv)[S]) {
@@ -226,23 +221,21 @@ __device__ __forceinline__ void depth_residual_half(const DevConsts& dc, const S
   if (run && (dc.td_nu + 1) * (double)nz < 0.95 * (double)N * (1.0 - 1e-9) && rmin > 1e-6) { sc2 = dc.td_scale2; run = false; }
   const double nu1 = dc.td_nu + 1, invN = 1.0 / (double)N;
   // Fast loop: both halves iterate together (a finished half keeps computing, its updates are masked).
-  if (IRLS == 1) {
-    // sum_i r_i^2 (nu+1) / (nu + r_i^2/s) == (nu+1) s sum_i a2_i / (nu s + a2_i), one reciprocal per four pixels.
-    while (__any_sync(FULL, run && sc1 > 1e-30)) {
-      const double nus = dc.td_nu * sc1, c1 = nu1 * sc1;
-      const double sum = c1 * half_sum(irls_lane_sum<S>(a2, nus));
-      if (run && sc1 > 1e-30) {
-        if (sum == 0) { sc2 = dc.td_scale2; run = false; }
-        else {
-          sc2 = sum * invN;
-          run = fabs(sc2 - sc1) > 0.05 * sc1;
-          sc1 = sc2;
-        }
+  // sum_i r_i^2 (nu+1) / (nu + r_i^2/s) == (nu+1) s sum_i a2_i / (nu s + a2_i), one reciprocal per four pixels.
+  while (__any_sync(FULL, run && sc1 > 1e-30)) {
+    const double nus = dc.td_nu * sc1, c1 = nu1 * sc1;
+    const double sum = c1 * half_sum(irls_lane_sum<S>(a2, nus));
+    if (run && sc1 > 1e-30) {
+      if (sum == 0) { sc2 = dc.td_scale2; run = false; }
+      else {
+        sc2 = sum * invN;
+        run = fabs(sc2 - sc1) > 0.05 * sc1;
+        sc1 = sc2;
       }
     }
   }
   // r^2 (nu+1) / (nu + r^2/s) == (r^2 (nu+1) s) / (nu s + r^2): one reciprocal per pixel, S independent chains.
-  // (With IRLS == 1 only the rare scales below 1e-30 get here.)
+  // Only the rare scales below 1e-30 get here.
   while (__any_sync(FULL, run && sc1 > 1e-250)) {
     const double nus = dc.td_nu * sc1, c1 = nu1 * sc1;
     double t[S];
@@ -338,16 +331,14 @@ __device__ __noinline__ double lmpar_1d(double r, double d, double q, double del
 }
 
 // S = residual slots per lane: 7 covers patches up to 112 pixels (the shipped 15x7), 8 up to kMaxPatch = 128.
-template <int S, int MB, bool TD, int IRLS>
-__global__ void __launch_bounds__(32, MB) lm_kernel(DevConsts dc, LmArgs a) {
+template <int S, bool TD>
+__global__ void __launch_bounds__(32, 16) lm_kernel(DevConsts dc, LmArgs a) {
   const int lane = threadIdx.x & 31, half = lane >> 4, hl = lane & 15;
   const int k = blockIdx.x;
   const int n = a.n_ptr ? (int)*a.n_ptr : a.n_fixed;
   if (k >= n) return;
   const esvo_seed& sd = a.seeds[k];
   const int m = dc.wx * dc.wy;
-  long long t_start = 0, glob_start = 0;
-  if (a.dbg) { t_start = clock64(); asm volatile("mov.u64 %0, %globaltimer;" : "=l"(glob_start)); }
   // Cold per-seed state is kept in shared memory so that the hot loops fit the register budget of MB seeds / SM:
   // the patch geometry (warp-uniform) and fcur, the accepted residual vectors (touched once per LM step).
   __shared__ SeedGeom g;
@@ -405,7 +396,7 @@ __global__ void __launch_bounds__(32, MB) lm_kernel(DevConsts dc, LmArgs a) {
       s_si[0] = nfev; s_si[1] = nexec; s_si[2] = iter; s_si[3] = iteration; s_si[4] = optState; s_si[5] = phase;
     }
     __syncwarp();
-    depth_residual_half<S, TD, IRLS>(dc, g, a.tl, a.tr, rho_e, off, vmask, fnew);
+    depth_residual_half<S, TD>(dc, g, a.tl, a.tr, rho_e, off, vmask, fnew);
     __syncwarp();
     x = s_st[0]; xn = s_st[1]; fnorm = s_st[2]; par = s_st[3]; diag = s_st[4]; delta = s_st[5]; xnorm = s_st[6];
     r00 = s_st[7]; qtf = s_st[8]; gnorm = s_st[9]; pstep = s_st[10]; pnorm = s_st[11];
@@ -530,7 +521,6 @@ __global__ void __launch_bounds__(32, MB) lm_kernel(DevConsts dc, LmArgs a) {
     const double inv = (r00 != 0.) ? (1. / r00) * (1. / r00) : 0.0;       // internal::covar, n = 1
     if (!TD && dc.lsnorm == ESVO_LSNORM_L2) var = (fnorm * fnorm / (m - 1)) * inv;   // :200-206
     else var = (dc.td_stdvar * dc.td_stdvar) * inv;                       // :207-211 (Tdist; zncc leaves it unset)
-    if (a.dbg) { long long ge; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(ge)); a.dbg[4 * k] = clock64() - t_start; a.dbg[4 * k + 1] = nfev; a.dbg[4 * k + 2] = ge - glob_start; a.dbg[4 * k + 3] = glob_start; }
     a.flag[k] = ok;
     a.res[3 * k] = x; a.res[3 * k + 1] = var; a.res[3 * k + 2] = fnorm * fnorm;      // :212
   }
@@ -545,14 +535,11 @@ __global__ void __launch_bounds__(32, MB) lm_kernel(DevConsts dc, LmArgs a) {
 // Here the per-slot phases are ROLLED loops (7 trips of ~60 / ~35 / ~25 instructions) that hand their per-lane values
 // over through shared memory (residuals r, the two residual vectors f(x) | f(x+h) double-buffered); only the scale
 // iteration keeps its seven squared residuals in registers.  Register pressure drops with it (no parking of the
-// solver state needed), so more seeds are resident per SM.
+// solver state needed), so more seeds are resident per SM.  The bilinear taps are per-lane LDG.E.U8 against L1 (97 % hit
+// rate); staging the source tiles in shared memory by TMA gained nothing (DESIGN.md §9).
 // --------------------------------------------------------------------------------------------
-// TMA = true (experiment, ESVO_LM_TMA=1): the two (wx+1) x (wy+1) source tiles of each half's evaluation are fetched by
-// cp.async.bulk.tensor.2d (box 32 x 8 from the 16-byte aligned column below the tile) into shared memory behind an mbarrier
-// and the bilinear taps read shared memory; TMA = false: per-lane LDG.E.U8 against L1 (97 % hit rate).  Same arithmetic.
-struct LmTmaMaps { CUtensorMap l, r; };
-template <int S, int MB, bool DBG = false, bool TMA = false>
-__global__ void __launch_bounds__(32, MB) lm2_kernel(DevConsts dc, LmArgs a, const __grid_constant__ LmTmaMaps tm) {
+template <int S, int MB>
+__global__ void __launch_bounds__(32, MB) lm2_kernel(DevConsts dc, LmArgs a) {
   const int lane = threadIdx.x & 31, half = lane >> 4, hl = lane & 15;
   const int k = blockIdx.x;
   const int n = a.n_ptr ? (int)*a.n_ptr : a.n_fixed;
@@ -565,9 +552,6 @@ __global__ void __launch_bounds__(32, MB) lm2_kernel(DevConsts dc, LmArgs a, con
   __shared__ int s_off[S * 16];
   __shared__ double s_r[S][32];
   __shared__ double s_f[2][S][32];
-  __shared__ __align__(128) uint8_t s_tile[TMA ? 2 : 1][TMA ? 2 : 1][TMA ? 256 : 16];   // [half][image][8 rows x 32 bytes]
-  __shared__ __align__(8) unsigned long long s_bar;
-  const int tpitch = TMA ? 32 : dc.pitch;          // row pitch the slot offsets are built for
   if (lane < 12) {
     const int r = lane >> 2, cidx = lane & 3;
     double s = 0;
@@ -579,13 +563,7 @@ __global__ void __launch_bounds__(32, MB) lm2_kernel(DevConsts dc, LmArgs a, con
   for (int q = lane; q < S * 16; q += 32) {
     const int s = q >> 4, kk = (q & 15) + 16 * s;
     const int py = kk / wx, px = kk - py * wx;
-    s_off[q] = kk < m ? py * tpitch + px : 0;
-  }
-  unsigned tma_parity = 0;
-  const unsigned bar_addr = (unsigned)__cvta_generic_to_shared(&s_bar);
-  if (TMA && lane == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 2;" ::"r"(bar_addr) : "memory");     // one arrival per half
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    s_off[q] = kk < m ? py * dc.pitch + px : 0;
   }
   __syncwarp();
   const double EPS = 2.220446049250313e-16;
@@ -604,8 +582,6 @@ __global__ void __launch_bounds__(32, MB) lm2_kernel(DevConsts dc, LmArgs a, con
   double xn = x, pstep = 0, pnorm = 0;
   int iteration = 0, optState = 0;
   int phase = 0, cur = 0;       // cur: which s_f buffer holds the accepted f(x) | f(x+h)
-  const long long t_start = DBG ? clock64() : 0;
-  int n_trips = 0;
   bool done = false;
   while (!done) {
     const double xe = (phase == 0) ? x : xn;
@@ -643,31 +619,14 @@ __global__ void __launch_bounds__(32, MB) lm2_kernel(DevConsts dc, LmArgs a, con
       const double q1b = (fx2 + 1) - x2, q2b = x2 - fx2, q3b = (fy2 + 1) - y2, q4b = y2 - fy2;
       const uint8_t* basea = a.tl + (size_t)uly1 * dc.pitch + ulx1;
       const uint8_t* baseb = a.tr + (size_t)uly2 * dc.pitch + ulx2;
-      if (TMA) {
-        // each half fetches its two tiles (box origin on the 16-byte aligned column at or below the tile, see bm_tma_kernel)
-        const int xa = ulx1 & ~15, xb = ulx2 & ~15;
-        if (hl == 0) {
-          const unsigned da = (unsigned)__cvta_generic_to_shared(&s_tile[half][0][0]), db = (unsigned)__cvta_generic_to_shared(&s_tile[half][1][0]);
-          asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_addr), "r"(512u) : "memory");
-          asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                       ::"r"(da), "l"(reinterpret_cast<unsigned long long>(&tm.l)), "r"(bar_addr), "r"(xa), "r"(uly1) : "memory");
-          asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                       ::"r"(db), "l"(reinterpret_cast<unsigned long long>(&tm.r)), "r"(bar_addr), "r"(xb), "r"(uly2) : "memory");
-        }
-        basea = &s_tile[half][0][0] + (ulx1 - xa);
-        baseb = &s_tile[half][1][0] + (ulx2 - xb);
-        unsigned done = 0;
-        while (!done) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.b32 %0, 1, 0, p; }" : "=r"(done) : "r"(bar_addr), "r"(tma_parity) : "memory");
-        tma_parity ^= 1u;
-      }
       // ---- phase A: residuals of the lane's slots (rolled) ----
 #pragma unroll 1
       for (int s = 0; s < S; ++s) {
         const int o = s_off[s * 16 + hl];
         const uint8_t* pa = basea + o;
         const uint8_t* pb = baseb + o;
-        const double a00 = pa[0], a01 = pa[1], a10 = pa[tpitch], a11 = pa[tpitch + 1];
-        const double b00 = pb[0], b01 = pb[1], b10 = pb[tpitch], b11 = pb[tpitch + 1];
+        const double a00 = pa[0], a01 = pa[1], a10 = pa[dc.pitch], a11 = pa[dc.pitch + 1];
+        const double b00 = pb[0], b01 = pb[1], b10 = pb[dc.pitch], b11 = pb[dc.pitch + 1];
         const double t1 = q3a * (q1a * a00 + q2a * a01) + q4a * (q1a * a10 + q2a * a11);
         const double t2 = q3b * (q1b * b00 + q2b * b01) + q4b * (q1b * b10 + q2b * b11);
         const bool on = ok && (s < n_valid);
@@ -690,7 +649,6 @@ __global__ void __launch_bounds__(32, MB) lm2_kernel(DevConsts dc, LmArgs a, con
       while (__any_sync(FULL, run && sc1 > 1e-30)) {
         const double nus = nu * sc1, c1 = nu1 * sc1;
         const double sum = c1 * half_sum(irls_lane_sum<S>(a2, nus));
-        if (DBG) ++n_trips;
         if (run && sc1 > 1e-30) {
           if (sum == 0) { sc2 = dc.td_scale2; run = false; }
           else { sc2 = sum * invN; run = fabs(sc2 - sc1) > 0.05 * sc1; sc1 = sc2; }
@@ -842,7 +800,6 @@ __global__ void __launch_bounds__(32, MB) lm2_kernel(DevConsts dc, LmArgs a, con
     const double inv = (r00 != 0.) ? (1. / r00) * (1. / r00) : 0.0;
     a.flag[k] = okx;
     a.res[3 * k] = x; a.res[3 * k + 1] = (dc.td_stdvar * dc.td_stdvar) * inv; a.res[3 * k + 2] = fnorm * fnorm;
-    if (DBG && a.dbg) { a.dbg[4 * k] = clock64() - t_start; a.dbg[4 * k + 1] = nfev; a.dbg[4 * k + 2] = nexec; a.dbg[4 * k + 3] = n_trips; }
   }
 }
 
@@ -947,44 +904,16 @@ int lm_run(Ctx* c, const esvo_seed* d_seeds, size_t n_fixed) {
   a.seeds = d_seeds; a.n_ptr = n_fixed ? nullptr : (const unsigned long long*)(c->d_counters + 1);
   a.n_fixed = (int)n_fixed; a.tl = c->obs_ls; a.tr = c->obs_rs; std::memcpy(a.T_left_world, c->T_left_world_inv, sizeof(a.T_left_world));
   a.flag = c->lm_flag; a.res = c->lm_res; a.counters = (unsigned long long*)c->d_counters;
-  a.dbg = c->lm_dbg;
   const int upper = (int)(n_fixed ? n_fixed : c->n_ev);
   if (upper == 0) return ESVO_OK;
-  // default: lm2_kernel, 20 seeds per SM.  On an H100 SXM (700 W limit; ESVO_LM_VARIANT=1<seeds>11 python bench.py --no-parity
-  // --no-extras --no-cpu-baseline) it beats 16 / 24 / 32 seeds per SM both as an isolated launch (0.62 vs 0.64 / 0.73 /
-  // 0.82 ms) and in the 16-slot pipeline (0.237 vs 0.240 / 0.238 / 0.257 ms/step).  Experiment switch: ESVO_LM_VARIANT = [1 = lm2]<seeds per SM><irls mode><td>,
-  // e.g. 1600 = the round-1 kernel, 1611 = + Tdist specialisation + grouped reciprocal, 12011 = lm2 with 20 seeds per SM
-  static const int variant = [] { const char* e = getenv("ESVO_LM_VARIANT"); return e ? atoi(e) : 12011; }();
-  const bool td = c->dc.lsnorm == ESVO_LSNORM_TDIST && (variant % 10);
-  const int irls = (variant / 10) % 10, mb = (variant / 100) % 100;
+  // Tdist with up to 7 slots per lane: lm2_kernel at 20 seeds per SM.  On an H100 SXM (700 W limit, bench.py --no-parity
+  // --no-extras --no-cpu-baseline) 20 beat 16 / 24 / 32 seeds per SM both as an isolated launch (0.62 vs 0.64 / 0.73 /
+  // 0.82 ms) and in the 16-slot pipeline (0.237 vs 0.240 / 0.238 / 0.257 ms/step); see DESIGN.md §4.
+  const bool td = c->dc.lsnorm == ESVO_LSNORM_TDIST;
   const bool s7 = c->dc.wx * c->dc.wy <= 7 * 16;
-  if (variant >= 10000 && c->dc.lsnorm == ESVO_LSNORM_TDIST && s7) {
-    const int mb2 = (variant / 100) % 100;
-    static const int lm_debug = getenv("ESVO_LM_DEBUG") ? 1 : 0;      // per-seed cycles / evaluations / IRLS trips (scripts/lm_tail_probe.py)
-    static const int lm_tma = getenv("ESVO_LM_TMA") ? atoi(getenv("ESVO_LM_TMA")) : 0;   // experiment: TMA-staged source tiles
-    LmTmaMaps tm;
-    std::memset(&tm, 0, sizeof(tm));
-    if (lm_tma && c->dc.wx <= 15 && c->dc.wy <= 7 && make_u8_tensor_map(&tm.l, c->obs_ls, c->dc.W, c->dc.H, c->dc.pitch, 32, 8) &&
-        make_u8_tensor_map(&tm.r, c->obs_rs, c->dc.W, c->dc.H, c->dc.pitch, 32, 8)) {
-      if (mb2 == 24) lm2_kernel<7, 24, false, true><<<upper, 32, 0, c->stream>>>(c->dc, a, tm);
-      else lm2_kernel<7, 20, false, true><<<upper, 32, 0, c->stream>>>(c->dc, a, tm);
-    }
-    else if (lm_debug) lm2_kernel<7, 20, true><<<upper, 32, 0, c->stream>>>(c->dc, a, tm);
-    else if (mb2 == 32) lm2_kernel<7, 32><<<upper, 32, 0, c->stream>>>(c->dc, a, tm);
-    else if (mb2 == 24) lm2_kernel<7, 24><<<upper, 32, 0, c->stream>>>(c->dc, a, tm);
-    else if (mb2 == 20) lm2_kernel<7, 20><<<upper, 32, 0, c->stream>>>(c->dc, a, tm);
-    else lm2_kernel<7, 16><<<upper, 32, 0, c->stream>>>(c->dc, a, tm);
-    c->launches += 1;
-    ESVO_CUDA_TRY(c, cudaGetLastError());
-    return ESVO_OK;
-  }
-#define LM_LAUNCH(S_, MB_, TD_, I_) lm_kernel<S_, MB_, TD_, I_><<<upper, 32, 0, c->stream>>>(c->dc, a)
-  if (!s7) { if (td) LM_LAUNCH(8, 16, true, 1); else LM_LAUNCH(8, 16, false, 1); }
-  else if (!td) { if (irls) LM_LAUNCH(7, 16, false, 1); else LM_LAUNCH(7, 16, false, 0); }
-  else if (mb == 24) { if (irls) LM_LAUNCH(7, 24, true, 1); else LM_LAUNCH(7, 24, true, 0); }
-  else if (mb == 20) { if (irls) LM_LAUNCH(7, 20, true, 1); else LM_LAUNCH(7, 20, true, 0); }
-  else { if (irls) LM_LAUNCH(7, 16, true, 1); else LM_LAUNCH(7, 16, true, 0); }
-#undef LM_LAUNCH
+  if (td && s7) lm2_kernel<7, 20><<<upper, 32, 0, c->stream>>>(c->dc, a);
+  else if (!s7) { if (td) lm_kernel<8, true><<<upper, 32, 0, c->stream>>>(c->dc, a); else lm_kernel<8, false><<<upper, 32, 0, c->stream>>>(c->dc, a); }
+  else lm_kernel<7, false><<<upper, 32, 0, c->stream>>>(c->dc, a);
   c->launches += 1;
   ESVO_CUDA_TRY(c, cudaGetLastError());
   return ESVO_OK;

@@ -18,8 +18,6 @@
 #include <algorithm>
 #include <cmath>
 
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace esvo {
@@ -809,8 +807,7 @@ ESVO_API int esvo_track_solve(esvo_ctx* c, int analytical, double Tout[16], esvo
   a.huber = p.trk_lsnorm == ESVO_TRK_LSNORM_HUBER; a.huber_thr = p.trk_huber_threshold; a.analytical = analytical != 0;
   a.state = t->d.state;
   const int smem = (TRK_MAXB * 6 + TRK_MAXB * 2 + TRK_MAXB * 3 + 16 * 8) * 8;
-  static const int trk_threads = [] { const char* e = getenv("ESVO_TRK_THREADS"); int v = e ? atoi(e) : TRK_THREADS; return (v >= 32 && v <= TRK_THREADS && v % 32 == 0) ? v : TRK_THREADS; }();
-  trk_solve_kernel<<<1, trk_threads, smem, c->stream>>>(c->dc, a);
+  trk_solve_kernel<<<1, TRK_THREADS, smem, c->stream>>>(c->dc, a);
   c->launches += 1;
   ESVO_CUDA_TRY(c, cudaGetLastError());
   double state[64];

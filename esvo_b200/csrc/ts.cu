@@ -442,8 +442,7 @@ static int ts_make_room(Ctx* c, int cam, size_t n_new) {
 // by the driver; callers that want true async overlap pass pinned buffers).
 // Host event packet whose four arrays are adjacent (at most 64 bytes of padding in total): start of the span, else null.
 static const uint8_t* packet_span(const uint16_t* x, const uint16_t* y, const int64_t* t, const uint8_t* p, size_t n, size_t& span) {
-  static const int enabled = getenv("ESVO_TS_PACKET_COPY") ? atoi(getenv("ESVO_TS_PACKET_COPY")) : 1;
-  if (!enabled || !p || n < 4096) return nullptr;                    // small pushes: the copies are not what costs
+  if (!p || n < 4096) return nullptr;                    // small pushes: the copies are not what costs
   const uint8_t* b[4] = {(const uint8_t*)x, (const uint8_t*)y, (const uint8_t*)t, p};
   const size_t len[4] = {n * 2, n * 2, n * 8, n};
   const uint8_t *lo = b[0], *hi = b[0] + len[0];

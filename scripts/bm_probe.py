@@ -1,5 +1,5 @@
 """BM kernel probe: esvo_bm_match on the bench workloads (hkust 5k events, dsec 20k events); prints the isolated kernel time
-(esvo_profile stage 1) and a digest of the seeds so that two runs (ESVO_BM_TMA=0/1) can be compared."""
+(esvo_profile stage 1) and a digest of the seeds so that two builds can be compared."""
 import ctypes as C, hashlib, os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -21,5 +21,5 @@ for rig, n, kw in (("hkust", 5000, {}), ("dsec", 20000, dict(n_segments=120))):
         m, c = (C.c_double * 8)(), (C.c_uint64 * 8)()
         g._call("profile_read", [f64, u64], m, c)
         ts.append(m[1])
-    print(f"{rig}: tma={os.environ.get('ESVO_BM_TMA', '0')} bm kernel {min(ts[1:]) * 1e3:.1f} us, seeds {seeds.size}, evals {ev}, digest {hashlib.md5(seeds.tobytes()).hexdigest()[:12]}")
+    print(f"{rig}: bm kernel {min(ts[1:]) * 1e3:.1f} us, seeds {seeds.size}, evals {ev}, digest {hashlib.md5(seeds.tobytes()).hexdigest()[:12]}")
     g.close()

@@ -1,6 +1,5 @@
 """Fusion-stage timing probe at pipeline depth 1: the bench frame's fusion (stage + order + fold + regularise + commit) alone,
-CUDA events of the library's profile stage 5; ESVO_DBG_FOLD_PHASE = 1 / 2 stops the fold after the list walk / after the sort
-(map contents are then garbage -- timing only).  usage: python scripts/fold_probe.py [cfg2|cfg3]"""
+CUDA events of the library's profile stage 5.  usage: python scripts/fold_probe.py [cfg2|cfg3]"""
 import ctypes as C, os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -31,5 +30,4 @@ for k in range(n_prime + 6):
         g._call("profile_read", [f64, u64], ms, cnt); g._call("profile", [C.c_int], 0)
         ts.append(list(ms)[:6])
 ts = np.array(ts)
-print(cfgname, "phase", os.environ.get("ESVO_DBG_FOLD_PHASE", "0"), "sort", os.environ.get("ESVO_FOLD_SORT", "1"),
-      "stage ms [ts, bm, seed order, lm, point order, fusion]:", np.round(np.median(ts, axis=0), 4).tolist(), "n_fusions", c["n_fusions"], "map", c["map_size"])
+print(cfgname, "stage ms [ts, bm, seed order, lm, point order, fusion]:", np.round(np.median(ts, axis=0), 4).tolist(), "n_fusions", c["n_fusions"], "map", c["map_size"])

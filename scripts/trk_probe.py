@@ -26,4 +26,4 @@ for analytical in (True, False):
         t0 = time.perf_counter(); g.track_reset(c, Tw, Tw, ts_cur); t1 = time.perf_counter(); T, st = g.track_solve(analytical); t2 = time.perf_counter()
         tt.append(((t1 - t0) * 1e3, (t2 - t1) * 1e3))
     tt = np.array(tt[2:])
-    print(f"threads {os.environ.get('ESVO_TRK_THREADS', 'default')} analytical={analytical}: reset {np.median(tt[:,0]):.3f} ms solve {np.median(tt[:,1]):.3f} ms stats {st} pose t {T[:3,3]}")
+    print(f"analytical={analytical}: reset {np.median(tt[:,0]):.3f} ms solve {np.median(tt[:,1]):.3f} ms stats {st} pose t {T[:3,3]}")
