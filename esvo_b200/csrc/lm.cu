@@ -104,6 +104,23 @@ __device__ __forceinline__ double irls_group2(double a0, double a1, double nus) 
   const double d0 = nus + a0, d1 = nus + a1;
   return fma(a0, d1, a1 * d0) * rcp_nr(d0 * d1);
 }
+// Degenerate regime of the reference's scale iteration (DepthProblem.cpp:96-119).  With m non-zero residuals of N the update
+//   s' = (1/N) sum_i r_i^2 (nu+1) / (nu + r_i^2/s)  <=  s (nu+1) m / N = c s,
+// so for c < 0.95 every exact step shrinks s by more than 5 %: s decays geometrically (thousands of passes) until r_i^2/s
+// overflows to +inf for every pixel, the sum becomes exactly 0 and :116-119 resets the scale to td_scale^2.  That is only
+// certain while rounding cannot pass the 5 % test: once s is subnormal (k steps of 2^-1074) a step's rounding error is below
+// one step, so the loop can stall where 0.95 eps k <= 1 (eps = 1 - c / 0.95).  The smallest residual keeps the sum non-zero
+// down to k = min r^2 / (DBL_MAX 2^-1074) = min r^2 / 2^-50, so the reset is proven when 0.95 eps min r^2 > 2^-50, i.e.
+//   gap min r^2 > 2^-50 N  with gap = 0.95 N - (nu+1) m;
+// the guard asks for twice that (DESIGN.md deviation 4).  The 1e-9 margin covers the rounding of steps at normal scales.
+constexpr double kIrlsResetGap = 0x1p-49;
+// r_min > 1e-6 alone proves the reset where gap >= kIrlsGapNoTiny N (eps >= 1.9e-3: every shipped shape at both shipped nu).
+constexpr double kIrlsGapNoTiny = kIrlsResetGap / 1e-12;
+__device__ __forceinline__ bool irls_degenerate(double nu1, int nz, int N) {
+  return nu1 * (double)nz < 0.95 * (double)N * (1.0 - 1e-9);
+}
+__device__ __forceinline__ double irls_gap(double nu1, int nz, int N) { return 0.95 * (double)N - nu1 * (double)nz; }
+
 template <int S>
 __device__ __forceinline__ double irls_lane_sum(const double (&a)[S], double nus) {
   double acc = 0.0;
@@ -207,19 +224,15 @@ __device__ __forceinline__ void depth_residual_half(const DevConsts& dc, const S
     a2[s] = r[s] * r[s];
     if (r[s] != 0) { nz++; rmin = fmin(rmin, fabs(r[s])); }
   }
-  // Degenerate regime of the reference's scale iteration.  With m non-zero residuals the update is
-  //   s' = (1/N) sum_i r_i^2 (nu+1) / (nu + r_i^2/s)  <=  s (nu+1) m / N,
-  // so for (nu+1) m / N < 0.95 every step shrinks s by more than 5 %: the loop at DepthProblem.cpp:96
-  // can never leave through its 5 % test, s decays geometrically (thousands of iterations) until
-  // r_i^2/s overflows to +inf for every pixel, the sum becomes exactly 0 and :116-119 resets the
-  // scale to td_scale^2.  We jump straight to that fixed outcome (see DESIGN.md "IRLS degenerate regime");
-  // the overflow argument needs every non-zero |r_i| to be far above sqrt(DBL_MAX * denorm_min) ~ 1e-8.
+  // Degenerate regime (irls_degenerate): jump straight to the reset where it is proven.
   nz = half_sum_i(nz);
   rmin = half_min(rmin);
+  const double nu1 = dc.td_nu + 1, invN = 1.0 / (double)N;
   double sc1 = dc.td_scale2, sc2 = -1.0;
   bool run = ok;
-  if (run && (dc.td_nu + 1) * (double)nz < 0.95 * (double)N * (1.0 - 1e-9) && rmin > 1e-6) { sc2 = dc.td_scale2; run = false; }
-  const double nu1 = dc.td_nu + 1, invN = 1.0 / (double)N;
+  if (run && irls_degenerate(nu1, nz, N) && irls_gap(nu1, nz, N) * (rmin * rmin) >= kIrlsResetGap * (double)N) {
+    sc2 = dc.td_scale2; run = false;
+  }
   // Fast loop: both halves iterate together (a finished half keeps computing, its updates are masked).
   // sum_i r_i^2 (nu+1) / (nu + r_i^2/s) == (nu+1) s sum_i a2_i / (nu s + a2_i), one reciprocal per four pixels.
   while (__any_sync(FULL, run && sc1 > 1e-30)) {
@@ -642,10 +655,23 @@ __global__ void __launch_bounds__(32, MB) lm2_kernel(DevConsts dc, LmArgs a) {
 #pragma unroll
       for (int s = 0; s < S; ++s) { const double r = s_r[s][lane]; a2[s] = r * r; }
       nz = half_sum_i(nz);
-      const bool no_tiny = ((__ballot_sync(FULL, tiny) >> (half * 16)) & 0xffffu) == 0;      // min |r| over the non-zero residuals > 1e-6
+      // Degenerate regime (irls_degenerate).  Far from the 0.95 threshold r_min > 1e-6 proves the reset; closer to it the half
+      // needs min r^2 itself.  Such a half votes with all its lanes, so one ballot serves both and the min reduction runs
+      // only when some half shows all 16 lanes set.
+      const bool deg = irls_degenerate(nu1, nz, m);
+      const double gap = irls_gap(nu1, nz, m);
+      const bool need_min = ok && deg && gap < kIrlsGapNoTiny * (double)m;
+      const unsigned vote = __ballot_sync(FULL, tiny || need_min);
+      const bool no_tiny = ((vote >> (half * 16)) & 0xffffu) == 0;      // min |r| over the non-zero residuals > 1e-6
+      double a2min = 1e300;
+      if ((vote & 0xffffu) == 0xffffu || (vote >> 16) == 0xffffu) {   // warp-uniform
+#pragma unroll
+        for (int s = 0; s < S; ++s) if (a2[s] != 0) a2min = fmin(a2min, a2[s]);
+        a2min = half_min(a2min);
+      }
       double sc1 = dc.td_scale2;
       bool run = ok;
-      if (run && nu1 * (double)nz < 0.95 * (double)m * (1.0 - 1e-9) && no_tiny) { sc2 = dc.td_scale2; run = false; }
+      if (run && deg && (need_min ? gap * a2min >= kIrlsResetGap * (double)m : no_tiny)) { sc2 = dc.td_scale2; run = false; }
       while (__any_sync(FULL, run && sc1 > 1e-30)) {
         const double nus = nu * sc1, c1 = nu1 * sc1;
         const double sum = c1 * half_sum(irls_lane_sum<S>(a2, nus));

@@ -340,7 +340,8 @@ static thread_local uint64_t g_irls_hist[8] = {0};  // non-degenerate evals by i
 static thread_local uint64_t g_irls_nd_iters = 0, g_irls_deg = 0;
 // TIMING AID ONLY (bench.py cpu_baseline.with_shortcut), default off so that parity stays literal: skip the reference's
 // degenerate scale iteration the way the CUDA kernel does (lm.cu "degenerate regime": with m non-zero residuals and
-// (nu+1) m / N < 0.95 the loop of DepthProblem.cpp:96 can only end through sum == 0 -> scale = td_scale^2).
+// (nu+1) m / N < 0.95 the loop of DepthProblem.cpp:96 ends through sum == 0 -> scale = td_scale^2 wherever the guard proves
+// that rounding at subnormal scales cannot pass its 5 % test first).
 static int g_irls_shortcut = 0;
 struct DepthProblem {
   const CameraSystem* cs = nullptr;
@@ -416,7 +417,8 @@ struct DepthProblem {
         if (g_irls_shortcut) {
           int nzs = 0; double rmin = 1e300;
           for (int i = 0; i < N; ++i) { vR[i] = tau1[i] - tau2[i]; vR2[i] = vR[i] * vR[i]; if (vR[i] != 0) { nzs++; rmin = std::min(rmin, std::fabs(vR[i])); } }
-          if ((td_nu + 1) * (double)nzs < 0.95 * (double)N * (1.0 - 1e-9) && rmin > 1e-6) { s2 = td_scale2; first = false; s1 = s2; }
+          const double nu1 = td_nu + 1, gap = 0.95 * (double)N - nu1 * (double)nzs;   // the kernels' guard, DESIGN.md deviation 4
+          if (nu1 * (double)nzs < 0.95 * (double)N * (1.0 - 1e-9) && gap * (rmin * rmin) >= 0x1p-49 * (double)N) { s2 = td_scale2; first = false; s1 = s2; }
         }
         while (std::fabs(s2 - s1) / s1 > 0.05 || first) {           // :96
           ++g_irls_iters; if (++loc > g_irls_max) g_irls_max = loc;

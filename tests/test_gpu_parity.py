@@ -275,8 +275,8 @@ def lm_kernel_for(lsnorm, wx, wy):
     patches the 8-slot lm_kernel; l2 and zncc run lm_kernel with 7 or 8 slots per lane by the same bound."""
     slots = 7 if wx * wy <= 7 * 16 else 8
     if lsnorm == capi.LSNORM_TDIST:
-        return "lm2_kernel<7,20>" if slots == 7 else "lm_kernel<8,16,true,1>"
-    return f"lm_kernel<{slots},16,false,1>"
+        return "lm2_kernel<7,20>" if slots == 7 else "lm_kernel<8,true>"
+    return f"lm_kernel<{slots},false>"
 
 
 _TD, _L2, _ZN = capi.LSNORM_TDIST, capi.LSNORM_L2, capi.LSNORM_ZNCC

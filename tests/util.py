@@ -616,3 +616,143 @@ def maps_bit_identical(mo, mg, tag, p_cam_rtol=1e-12):
     fin = np.isfinite(pc_o)
     assert np.array_equal(fin, np.isfinite(pc_g)), tag + ": p_cam finiteness"
     assert np.allclose(pc_g[fin], pc_o[fin], rtol=p_cam_rtol, atol=1e-300), (tag, "p_cam", np.abs(pc_g[fin] - pc_o[fin]).max())
+
+
+# ---- depth LM, Student-t scale iteration: one hand-built case table for the CPU restatement (tests/test_depth_irls_pins.py)
+# and the device parity (tests/test_gpu_depth_irls.py).  Every case runs on the hkust rig with T_world_left =
+# T_world_virtual = identity.  The right time surface is the left one shifted by D pixels; the seed sits at (x + 0.5, y) with
+# y a whole row, so the lower tap row has weight exactly 0 and every patch row is independent; its inverse depth puts the
+# right patch delta pixels off, so pixel k's residual is delta * g_k for the integer horizontal gradient g_k the case draws
+# (the image values stay within 0..63, so the taps of zero gradients cancel exactly).  nz and min |r| are thus chosen, and
+# nu places c = (nu+1) nz / N against 0.95 (eps = 1 - c / 0.95).  big = (E, k): the right surface is raised by E under the
+# first k pixels, residuals of about -E among the small ones.
+DEPTH_DEFAULT = dict(patch=(15, 7), nz=28, g=1, delta=1.5e-6, nu=2.182, scale=17.277, eps=None, ulp=0, big=None, D=10, x=100,
+                     y=130, edge=False)
+
+
+def _dc(name, **kw):
+    c = dict(DEPTH_DEFAULT, **kw)
+    c["id"] = name
+    N = c["patch"][0] * c["patch"][1]
+    if c.get("below_095"):                               # the largest nu with (nu+1) nz < 0.95 N: inside the 1e-9 margin
+        nz, T = c["below_095"], 0.95 * float(N)
+        nu = T / nz - 1.0
+        while (nu + 1) * float(nz) >= T:
+            nu = float(np.nextafter(nu, -np.inf))
+        c["nu"] = nu
+    elif c["eps"] is not None or c["ulp"]:               # nu with (nu+1) nz = 0.95 N (1 - eps), or on the 1e-9 margin +- ulps
+        nz = c["nz"]
+        if c["eps"] is not None:
+            c["nu"] = 0.95 * N * (1.0 - c["eps"]) / nz - 1.0
+        else:
+            T = 0.95 * float(N) * (1.0 - 1e-9)
+            nu = T / nz - 1.0
+            while (nu + 1) * float(nz) < T:
+                nu = float(np.nextafter(nu, np.inf))
+            while (nu + 1) * float(nz) >= T:
+                nu = float(np.nextafter(nu, -np.inf))
+            # nu is now the largest value the guard's "<" accepts; ulp = +1 is the first it declines
+            c["nu"] = nu if c["ulp"] < 0 else float(np.nextafter(nu, np.inf))
+            c["ulp_at"] = c["ulp"]
+    return c
+
+
+DEPTH_CASES = [
+    # the shipped shape and both shipped nu (c = 0.85): the shortcut's common path, and non-degenerate controls
+    _dc("15x7-shipped-dsec"), _dc("15x7-shipped-hkust", nu=2.1897, scale=16.6397),
+    _dc("15x7-nondeg-1pass", nz=105, big=(17, 105), delta=1e-3), _dc("15x7-nondeg-2pass", nz=105, big=(16, 105), delta=1e-3),
+    _dc("15x7-nondeg-4pass", nz=105, big=(2, 105), delta=1e-3), _dc("15x7-c-above-0.95", nz=32, delta=1e-3),
+    _dc("15x7-mixed-big-tiny", nz=40, big=(40, 10), delta=1e-6),
+    # the band of the issue: 67 x 1 and 1 x 67 with 20 unit gradients at the shipped dsec nu (eps = 1.6e-4)
+    _dc("67x1-band-1.5e-6", patch=(67, 1), nz=20), _dc("67x1-reset-3e-6", patch=(67, 1), nz=20, delta=3e-6),
+    _dc("67x1-rmin-0.99e-6", patch=(67, 1), nz=20, delta=0.99e-6), _dc("67x1-rmin-1.01e-6", patch=(67, 1), nz=20, delta=1.01e-6),
+    _dc("1x67-band-1.5e-6", patch=(1, 67), nz=20, x=30, y=100), _dc("67x1-rmin-1e-4", patch=(67, 1), nz=20, delta=1e-4),
+    # a stall whose last subnormal step shrinks the scale by exactly 1/20: the division arm's "> 0.05" ends the loop there
+    _dc("67x1-stall-at-exact-5pct", patch=(67, 1), nz=20, delta=1.001500500166722e-06),
+    # eps placed at 1e-8 .. 1e-2 at N = 105, nz = 32, r_min = 3e-6; the 1e-9 margin itself and one ulp above it
+    *[_dc(f"15x7-eps{e:g}", nz=32, delta=3e-6, eps=e) for e in (1e-8, 1e-6, 1e-4, 1e-3, 1e-2)],
+    _dc("15x7-eps1e-6-rmin1.2e-6", nz=32, delta=1.2e-6, eps=1e-6), _dc("15x7-eps1e-6-rmin1e-5", nz=32, delta=1e-5, eps=1e-6),
+    _dc("15x7-eps1e-8-rmin1e-4", nz=32, delta=1e-4, eps=1e-8),
+    _dc("15x7-margin-accepted", nz=32, delta=3e-6, ulp=-1), _dc("15x7-margin-declined", nz=32, delta=3e-6, ulp=1),
+    # c one ulp below 0.95, inside the 1e-9 margin, with residuals of about -10 on 33 pixels: gap * min r^2 passes the reset bound,
+    # but the literal loop ends through a 5 % test decided at rounding level near a scale of 1e-15 (no reset)
+    _dc("15x7-inside-margin-big", nz=0, big=(10, 32), below_095=33),
+    # residuals below the old guard's 1e-6: the device's literal loops
+    _dc("15x7-rmin-1e-7", delta=1e-7), _dc("15x7-rmin-1e-8", delta=1e-8),
+    # lm2_kernel at m < 16 and lm_kernel<8, true> at 113, 121 and 127 pixels
+    _dc("1x1-nondeg", patch=(1, 1), nz=1, delta=1e-3), _dc("3x3-deg", patch=(3, 3), nz=2, delta=1e-5),
+    _dc("3x3-band", patch=(3, 3), nz=2, delta=3e-6, eps=1e-6),
+    _dc("113x1-band", patch=(113, 1), nz=32, delta=3e-6, eps=1e-6, x=110), _dc("113x1-shipped-nu", patch=(113, 1), nz=30, x=110),
+    _dc("11x11-band", patch=(11, 11), nz=36, delta=3e-6, eps=1e-6), _dc("11x11-shipped-nu", patch=(11, 11), nz=30),
+    _dc("127x1-band", patch=(127, 1), nz=36, delta=3e-6, eps=1e-6, x=110), _dc("127x1-eps1e-3", patch=(127, 1), nz=36, delta=3e-6, eps=1e-3, x=110),
+    # the right patch against the image's left edge: the warp holds at x0 and fails at x0 + h
+    _dc("15x7-warp-fails-at-x0+h", edge=True),
+]
+assert len({c["id"] for c in DEPTH_CASES}) == len(DEPTH_CASES)
+DEPTH_CASES = {c["id"]: c for c in DEPTH_CASES}
+
+
+def depth_params(c, lib, max_iteration=10):
+    p = configs.params_for("hkust", lib)
+    p.lsnorm = capi.LSNORM_TDIST
+    p.patch_size_x, p.patch_size_y = c["patch"]
+    p.td_nu, p.td_scale = c["nu"], c["scale"]
+    p.max_iteration = max_iteration
+    return p
+
+
+@functools.lru_cache(maxsize=None)
+def depth_inputs(cid):
+    """(tl, tr, seed, x_seed, y_seed) of DEPTH_CASES[cid]: the time surfaces, one seed (SEED_DTYPE) and its pixel position."""
+    import indep_depth as idp
+    c = DEPTH_CASES[cid]
+    A = configs.rig_arrays("hkust")
+    W, H = A["width"], A["height"]
+    Pl, Pr = A["left"]["P"], A["right"]["P"]
+    wx, wy = c["patch"]
+    hx, hy = (wx - 1) // 2, (wy - 1) // 2
+    N, D = wx * wy, c["D"]
+    x, y = c["x"], c["y"]
+    fb = -Pr[0][3]
+    if c["edge"]:
+        x = hx + D                                         # right patch centre 5e-8 px right of hx: x0 + h moves it 1.6e-7 px left
+        rho0 = (x + 0.5 - hx - 5e-8) / fb
+    else:
+        rho0 = (D + c["delta"]) / fb
+    # the inverse depth nearest rho0 at which the kernels' closed-form cam2World and the reference's literal one agree to the bit
+    cand = [rho0]
+    for k in range(1, 200):
+        cand += [_nx(rho0, k), _nx(rho0, -k)]
+    rho = None
+    for r in cand:
+        pd, pl = idp.cam2world_device(Pl, x + 0.5, float(y), r), idp.cam2world_literal(Pl, x + 0.5, float(y), r)
+        a1, a2 = idp.project(Pl, pd), idp.project(Pr, pd)
+        if a1 == idp.project(Pl, pl) and a2 == idp.project(Pr, pl) and a1 == (x + 0.5, float(y)):
+            rho = r
+            break
+    assert rho is not None, cid
+    # per-pixel gradients: nz pixels spread evenly over the patch (row-major), sign alternating along each row
+    g = np.zeros(N, np.int64)
+    g[np.round(np.linspace(0, N - 1, c["nz"])).astype(int) if c["nz"] else []] = c["g"]
+    g = g.reshape(wy, wx)
+    L = np.full((H, W), 32, np.int64)
+    ulx, uly = x - hx, y - hy
+    for py in range(wy):
+        row = uly + py
+        for px in range(wx):
+            s = 1 if px % 2 == 0 else -1
+            L[row, ulx + px + 1] = L[row, ulx + px] + s * g[py, px]
+        L[row, ulx + wx + 1:] = L[row, ulx + wx]
+    assert L.min() >= 0 and L.max() <= 63
+    R = np.full_like(L, 32)
+    R[:, :W - D] = L[:, D:]
+    if c["big"]:
+        E, k = c["big"]
+        for q in range(k):
+            py, px = divmod(q, wx)
+            R[uly + py, ulx - D + px:ulx - D + px + 2] = L[uly + py, ulx + px:ulx + px + 2] + E
+    seed = np.zeros(1, capi.SEED_DTYPE)
+    seed["x_left"] = seed["x_left_raw"] = (x + 0.5, float(y))
+    seed["T_world_virtual"] = np.eye(4).ravel()
+    seed["inv_depth"] = rho
+    return L.astype(np.uint8), R.astype(np.uint8), seed, x + 0.5, float(y)
