@@ -447,16 +447,29 @@ ESVO_API int esvo_ts_build(esvo_ctx* c, int cam, int64_t T, int64_t* idx_out, ui
   StreamScope sc(c, c->s_tsc[cam]);
   if (idx_out) ESVO_CUDA_TRY(c, cudaMemcpyAsync(idx_out, s.out_idx, (size_t)d.W * d.H * 8, cudaMemcpyDeviceToHost, c->stream));
   if (ts_out) ESVO_CUDA_TRY(c, cudaMemcpy2DAsync(ts_out, d.W, s.img_out, d.pitch, d.W, d.H, cudaMemcpyDeviceToHost, c->stream));
-  int32_t flags[4] = {0, 0, 0, 0};
+  int32_t flags[12] = {0};
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(flags, s.scalars, sizeof(flags), cudaMemcpyDeviceToHost, c->stream));
   ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   if (flags[1]) { c->set_error("events were not pushed in time order (unsupported on the device path)"); return ESVO_ERR_UNSUPPORTED; }
+  long long fold_t;                                      // stamp of the newest event folded out of the resident log (ts_make_room)
+  std::memcpy(&fold_t, flags + 10, 8);
+  if (s.log_base > 0 && (long long)T <= fold_t) {
+    c->set_error("t_sync " + std::to_string((long long)T) + " is not newer than the events folded out of the resident log; the oldest answerable t_sync is " +
+                 std::to_string(fold_t + 1));
+    return ESVO_ERR_UNSUPPORTED;
+  }
   return ESVO_OK;
 }
 ESVO_API int esvo_ts_set_unordered_input(esvo_ctx* c, int cam, int enable) {
   CHECK_CTX(c);
   if (cam < 0 || cam > 1) return ESVO_ERR_INVALID_ARG;
-  c->ts[cam].unordered = enable != 0;
+  TsState& s = c->ts[cam];
+  // the scan carries events_.back() from push to push; ordered pushes do not record it, so the switch cannot be turned on over them
+  if (enable && !s.unordered && (s.log_n || s.log_base)) {
+    c->set_error("esvo_ts_set_unordered_input: the camera already holds events pushed as ordered input; call esvo_ts_reset first");
+    return ESVO_ERR_UNSUPPORTED;
+  }
+  s.unordered = enable != 0;
   return ESVO_OK;
 }
 ESVO_API int esvo_ts_reset(esvo_ctx* c, int cam) {

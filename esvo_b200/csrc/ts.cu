@@ -426,8 +426,11 @@ static int ts_make_room(Ctx* c, int cam, size_t n_new) {
   unsigned g = (unsigned)((drop + B - 1) / B);
   ts_scatter_kernel<<<g, B, 0, c->stream>>>(s.ex, s.ey, s.et, drop, s.log_base, c->dc.W, c->dc.H, (long long*)s.base_idx,
                                             s.scalars + 8, (long long*)(s.max_t));
+  // scalars[10..11] (one int64): stamp of the newest folded event.  A build at T <= that stamp cannot be answered any more
+  // (folded events with t >= T are neither counted against the queue length nor skipped); esvo_ts_build refuses it.
   ts_scatter_fix_kernel<<<g, B, 0, c->stream>>>(s.ex, s.ey, s.et, s.ep, drop, s.log_base, c->dc.W, c->dc.H,
-                                                (const long long*)s.base_idx, (long long*)s.base_t, s.base_pol, nullptr);
+                                                (const long long*)s.base_idx, (long long*)s.base_t, s.base_pol,
+                                                (long long*)(s.scalars + 10));
   c->launches += 2;
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(s.ex2, s.ex + drop, keep * 2, cudaMemcpyDeviceToDevice, c->stream));
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(s.ey2, s.ey + drop, keep * 2, cudaMemcpyDeviceToDevice, c->stream));

@@ -187,13 +187,24 @@ ESVO_API int esvo_ts_push_events(esvo_ctx* ctx, int cam, const uint16_t* x, cons
  * (esvo_time_surface/src/TimeSurface.cpp:410-422); for time-ordered input that is the new event itself.  With
  * enable = 1 pushes of this camera go through a device prefix scan (running arg-max of the stamps) that reproduces
  * this for arbitrary input order, at the cost of two extra kernels per push.  With enable = 0 (default) input must be
- * time-ordered; a violation is detected on the device and reported by esvo_ts_build as ESVO_ERR_UNSUPPORTED. */
+ * time-ordered; a violation is detected on the device and reported by esvo_ts_build as ESVO_ERR_UNSUPPORTED (the
+ * flag stays up until esvo_ts_reset).
+ * The scan carries events_.back() from push to push, and ordered pushes do not record it.  So enable = 1 is accepted
+ * only while the camera holds no events (after esvo_create or esvo_ts_reset); on a camera that already took ordered
+ * pushes it returns ESVO_ERR_UNSUPPORTED and changes nothing. */
 ESVO_API int esvo_ts_set_unordered_input(esvo_ctx* ctx, int cam, int enable);
 
 /* replaces: TimeSurface::createTimeSurfaceAtTime (TimeSurface.cpp:52-152) incl.
  * EventQueueMat::getMostRecentEventBeforeT (TimeSurface.h:52-75).
  * idx_grid_out (H*W, may be NULL): index, in push order since create/reset, of the event each
- * pixel's value was taken from, -1 if none.  ts_out (H*W, may be NULL): the published mono8 image. */
+ * pixel's value was taken from, -1 if none.  ts_out (H*W, may be NULL): the published mono8 image.
+ * How far back t_sync_ns may lie: each camera keeps its newest events resident (4 Mi; when a push would overflow
+ * that, all but the newest 1 Mi are folded into one most-recent-event grid, so at least 1 Mi events are always
+ * resident).  The folded events' queues are gone, so t_sync_ns must be newer than the newest folded stamp:
+ * otherwise esvo_ts_build returns ESVO_ERR_UNSUPPORTED and esvo_last_error names the oldest t_sync_ns it can answer.
+ * The reference answers such a time from its 20-deep queues; this library does not guess.  esvo_run_ts_build does
+ * not read the device flags back and reports neither this nor an order violation.
+ * median_blur_kernel_size > 1 is not implemented: ESVO_ERR_UNSUPPORTED. */
 ESVO_API int esvo_ts_build(esvo_ctx* ctx, int cam, int64_t t_sync_ns, int64_t* idx_grid_out,
                            uint8_t* ts_out);
 ESVO_API int esvo_ts_reset(esvo_ctx* ctx, int cam);

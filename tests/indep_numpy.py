@@ -434,35 +434,114 @@ def vemp_to_points(matches, Pl, age_vis_threshold):
     return out
 
 
+# ---- a1: TimeSurface::eventsCallback (esvo_time_surface/src/TimeSurface.cpp:403-425) ----
+def events_callback_queue(ev):
+    """ev: dict of x, y, t (ns), p in ARRIVAL order, any stamp order.  Returns the same dict shape holding, per arrival, the event
+    the callback hands to insertEvent: events_.back() after the new event has been insertion-sorted into events_."""
+    events = []                                                                           # events_
+    out = []
+    for e in zip(ev["x"].tolist(), ev["y"].tolist(), ev["t"].tolist(), ev["p"].tolist()):
+        events.append(e)                                                                  # :412
+        i = len(events) - 2                                                               # :413
+        while i >= 0 and events[i][2] > e[2]:                                             # :414, strict: e goes after equal stamps
+            events[i + 1] = events[i]
+            i -= 1
+        events[i + 1] = e                                                                 # :419
+        out.append(events[-1])                                                            # :421 events_.back()
+    # clearEventQueue (:427-435) erases from the FRONT of events_ once it holds more than 5 000 000 entries; back() is never removed
+    a = np.array(out, dtype=np.int64).reshape(-1, 4)
+    return dict(x=a[:, 0].astype(np.uint16), y=a[:, 1].astype(np.uint16), t=a[:, 2].copy(), p=a[:, 3].astype(np.uint8))
+
+
 # ---- a1/a2: EventQueueMat (esvo_time_surface/include/esvo_time_surface/TimeSurface.h:28-96) and
-#      TimeSurface::createTimeSurfaceAtTime, BACKWARD mode (esvo_time_surface/src/TimeSurface.cpp:52-152); image ops by OpenCV itself
-def time_surface_backward(ev, T_ns, decay_ms, W, H, ignore_polarity, median_blur_kernel_size, map1, map2, queue_len=20):
-    """ev: dict of x, y, t (ns), p in ARRIVAL order.  Returns (raw mono8 before remap, published mono8 after remap)."""
-    import collections
-    import cv2
-    queues = collections.defaultdict(lambda: collections.deque(maxlen=queue_len))       # insertEvent: push_back, pop_front beyond queueLen
-    for x, y, t, p in zip(ev["x"].tolist(), ev["y"].tolist(), ev["t"].tolist(), ev["p"].tolist()):
-        if 0 <= x < W and 0 <= y < H:
-            queues[(x, y)].append((t, p))
+#      TimeSurface::createTimeSurfaceAtTime (esvo_time_surface/src/TimeSurface.cpp:52-152); image ops by OpenCV itself
+def _queue_walk(ev_effective, T_ns, decay_ms, W, H, ignore_polarity, queue_len):
+    """insertEvent for every arrival (ev_effective: what eventsCallback queued, in arrival order), then getMostRecentEventBeforeT
+    and the decayed value per pixel.  Returns [(y, x, value)] in raster order and the grid of the arrival number each came from."""
+    x = np.asarray(ev_effective["x"], np.int64); y = np.asarray(ev_effective["y"], np.int64)
+    t = np.asarray(ev_effective["t"], np.int64); p = np.asarray(ev_effective["p"])
+    arrival = np.nonzero((x < W) & (y < H))[0]                                            # insideImage; the others are never queued
+    pix = y[arrival] * W + x[arrival]
+    order = np.argsort(pix, kind="stable")                                                # per pixel, arrivals in push_back order
+    sp = pix[order]
+    from_back = np.searchsorted(sp, sp, side="right") - 1 - np.arange(sp.size)            # 0 = the queue's back()
+    queued = arrival[order]
+    # pop_front beyond queueLen leaves the last queue_len arrivals; the reverse walk of getMostRecentEventBeforeT returns the one
+    # nearest the back with ts < T, i.e. the largest arrival number among them
+    ok = (from_back < queue_len) & (t[queued] < T_ns)
+    best = np.full(W * H, -1, np.int64)
+    np.maximum.at(best, sp[ok], queued[ok])
     decay_sec = decay_ms / 1000.0
-    m = np.zeros((H, W), np.float64)
-    for (x, y), q in queues.items():
-        for t, p in reversed(q):                                                          # getMostRecentEventBeforeT: newest first, ts < T
-            if t < T_ns:
-                if ros_to_sec(t) > 0:
-                    d = T_ns - t                                                          # ros::Duration (integer ns), then toSec()
-                    dt = float(d // 1000000000) + 1e-9 * float(d % 1000000000)
-                    v = np.exp(-dt / decay_sec)
-                    if not ignore_polarity:
-                        v *= 1.0 if p else -1.0
-                    m[y, x] = v
-                break
-    m = 255.0 * m if ignore_polarity else 255.0 * (m + 1.0) / 2.0
+    hits = []
+    idx = np.full((H, W), -1, np.int64)
+    for q in np.nonzero(best >= 0)[0].tolist():                                           # ascending = the loops of :65-67, y outer, x inner
+        i = int(best[q])
+        ti = int(t[i])
+        if not ros_to_sec(ti) > 0:                                                        # :73
+            continue
+        d = int(T_ns) - ti                                                                # ros::Duration (integer ns), then toSec()
+        dt = float(d // 1000000000) + 1e-9 * float(d % 1000000000)
+        v = np.exp(-dt / decay_sec)
+        if not ignore_polarity:
+            v *= 1.0 if p[i] else -1.0
+        hits.append((q // W, q % W, float(v)))
+        idx[q // W, q % W] = i
+    return hits, idx
+
+
+def _to_mono8(m, ignore_polarity, median_blur_kernel_size):
+    import cv2
+    m = 255.0 * m if ignore_polarity else 255.0 * (m + 1.0) / 2.0                         # :123-126
     img = np.clip(np.rint(m), 0, 255).astype(np.uint8)                                    # convertTo(CV_8U): saturate_cast(cvRound), half to even
     if median_blur_kernel_size > 0:
-        img = cv2.medianBlur(img, 2 * median_blur_kernel_size + 1)
-    out = cv2.remap(img, map1, map2, cv2.INTER_LINEAR)
+        img = cv2.medianBlur(img, 2 * median_blur_kernel_size + 1)                        # :130-131
+    return img
+
+
+def time_surface_backward(ev, T_ns, decay_ms, W, H, ignore_polarity, median_blur_kernel_size, map1, map2, queue_len=20, info=None):
+    """ev: dict of x, y, t (ns), p in ARRIVAL order -- for out-of-order stamps the output of events_callback_queue.
+    Returns (raw mono8 before remap, published mono8 after remap); info["idx"]: arrival number behind every pixel, -1 if none."""
+    import cv2
+    hits, idx = _queue_walk(ev, T_ns, decay_ms, W, H, ignore_polarity, queue_len)
+    m = np.zeros((H, W), np.float64)
+    for y, x, v in hits:
+        m[y, x] = v                                                                       # :82-83
+    img = _to_mono8(m, ignore_polarity, median_blur_kernel_size)
+    out = cv2.remap(img, map1, map2, cv2.INTER_LINEAR)                                    # :149
+    if info is not None:
+        info["idx"] = idx
     return img, out
+
+
+def time_surface_forward(ev_effective, T_ns, decay_ms, W, H, ignore_polarity, median_blur_kernel_size, lut, queue_len=20, info=None):
+    """FORWARD mode (TimeSurface.cpp:86-116): every raw pixel, in raster order, splats its value onto the four neighbours of its
+    rectified point (lut: H x W x 2, precomputed_rectified_points_), each of the four sums clamped at 1 right away and never from
+    below.  The published image is this map as mono8 after the median; there is no remap (:138-142).  info: idx grid, the number
+    of clamps that fired and the smallest map value before conversion."""
+    hits, idx = _queue_walk(ev_effective, T_ns, decay_ms, W, H, ignore_polarity, queue_len)
+    lut = np.asarray(lut, np.float64).reshape(H, W, 2)
+    m = np.zeros((H, W), np.float64)
+    clamps = 0
+    for y, x, e in hits:
+        u, v = float(lut[y, x, 0]), float(lut[y, x, 1])
+        if not (u >= 0 and v >= 0):                                                       # :90 (false for NaN)
+            continue
+        u_i, v_i = int(np.floor(u)), int(np.floor(v))                                     # :92-93, size_t
+        if not (u_i + 1 < W and v_i + 1 < H):                                             # :95
+            continue
+        fu, fv = u - u_i, v - v_i
+        fu1, fv1 = 1.0 - fu, 1.0 - fv
+        m[v_i, u_i] += fu1 * fv1 * e                                                      # :101-104
+        m[v_i, u_i + 1] += fu * fv1 * e
+        m[v_i + 1, u_i] += fu1 * fv * e
+        m[v_i + 1, u_i + 1] += fu * fv * e
+        for yy, xx in ((v_i, u_i), (v_i, u_i + 1), (v_i + 1, u_i), (v_i + 1, u_i + 1)):  # :106-113
+            if m[yy, xx] > 1:
+                m[yy, xx] = 1
+                clamps += 1
+    if info is not None:
+        info.update(idx=idx, clamps=clamps, min_map=float(m.min()))
+    return _to_mono8(m, ignore_polarity, median_blur_kernel_size)
 
 
 # ---- a4: EventBM::match_an_event / match_all_HyperThread / match (esvo_core/src/core/EventBM.cpp:80-168,269-315) ----

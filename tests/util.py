@@ -756,3 +756,406 @@ def depth_inputs(cid):
     seed["T_world_virtual"] = np.eye(4).ravel()
     seed["inv_depth"] = rho
     return L.astype(np.uint8), R.astype(np.uint8), seed, x + 0.5, float(y)
+
+
+# ---- time-surface cases: push / build scripts that reach every branch of ts_push and ts_run_build (esvo_b200/csrc/ts.cu) ----
+# A case is (size, parameter tweak, script).  The script is a list of ops run on the oracle and on the product alike:
+#   ("push", how, ev)          how: host | nopol | dev | devnopol | packet (four adjacent host arrays) | packetnopol (three, pol = NULL)
+#   ("build", T)               index grid and image of both sides must be equal
+#   ("refused", T, code)       the product's esvo_ts_build must return `code`
+#   ("push_refused", ev, code) the product's push must return `code`; nothing is pushed on either side
+#   ("sync",) ("reset",)       esvo_sync (product) / esvo_ts_reset (both)
+#   ("unordered", on)          esvo_ts_set_unordered_input (product; the oracle always handles any order)
+#   ("unordered_refused",)     switching it on must return ESVO_ERR_UNSUPPORTED
+#   ("fresh", ev, T)           a new product context fed ev must build at T what this one built last
+TS_UNSUPPORTED, TS_CAPACITY = -6, -4
+TS_LOG_CAP = 1 << 22                       # resident events per camera (ts_alloc); a fold keeps TS_LOG_CAP / 4
+TS_EPOCH = 1_600_000_000_000_000_000       # a UNIX-epoch stamp in ns: 2.4e-7 s between neighbouring doubles
+TS_SIZES = {"hkust": (346, 260), "dsec": (640, 480), "small": (120, 96), "odd": (223, 165)}
+
+
+def ts_rig(size):
+    """Name under configs.RIGS: the shipped rigs, the small rig of the golden vectors, and hkust scaled to 223 x 165 (W % 32 = 31,
+    H % 8 = 5: partial tiles on both axes of the 32 x 8 raster kernels)."""
+    if size == "small" and "golden_small" not in configs.RIGS:
+        import ast
+        import os
+        z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "small_rig_frame.npz"), allow_pickle=False)
+        configs.RIGS["golden_small"] = ast.literal_eval(bytes(z["rig_json"]).decode())
+    if size == "odd" and "hkust_odd" not in configs.RIGS:
+        W, H = TS_SIZES["odd"]
+        h = configs.RIGS["hkust"]
+        sx, sy = W / h["width"], H / h["height"]
+        def scaled(c):
+            K = np.array(c["K"], float).reshape(3, 3); P = np.array(c["P"], float).reshape(3, 4)
+            K[0] *= sx; K[1] *= sy; P[0] *= sx; P[1] *= sy
+            return dict(K=K.ravel().tolist(), D=c["D"], R=c["R"], P=P.ravel().tolist())
+        configs.RIGS["hkust_odd"] = dict(width=W, height=H, model="plumb_bob", left=scaled(h["left"]), right=scaled(h["right"]))
+    return {"small": "golden_small", "odd": "hkust_odd"}.get(size, size)
+
+
+def ts_ev(x, y, t, p=None):
+    x = np.asarray(x, np.uint16)
+    return dict(x=x, y=np.asarray(y, np.uint16), t=np.asarray(t, np.int64), p=np.ones(x.size, np.uint8) if p is None else np.asarray(p, np.uint8))
+
+
+def ts_cut(ev, a, b):
+    return {k: v[a:b] for k, v in ev.items()}
+
+
+def ts_cat(*evs):
+    return {k: np.concatenate([e[k] for e in evs]) for k in ("x", "y", "t", "p")}
+
+
+def ts_random_stream(W, H, n, seed, t0=1_000_000_000, dt=2000):
+    """Time-ordered (equal stamps allowed); half of the events fall on a 24 x 16 patch, so its pixels hold more than any queue."""
+    rng = np.random.default_rng(seed)
+    x = rng.integers(0, W, n); y = rng.integers(0, H, n)
+    hot = rng.random(n) < 0.5
+    x[hot] = W // 3 + rng.integers(0, 24, hot.sum()); y[hot] = H // 3 + rng.integers(0, 16, hot.sum())
+    return ts_ev(x, y, t0 + np.cumsum(rng.integers(0, 2 * dt, n)), rng.integers(0, 2, n))
+
+
+def ts_jitter(ev, seed, frac=0.08, max_ns=2_000_000):
+    """A fraction of the events arrives with a stamp up to max_ns in the past."""
+    rng = np.random.default_rng(seed)
+    t = ev["t"].copy()
+    late = rng.random(t.size) < frac
+    late[0] = False
+    t[late] -= rng.integers(1_000, max_ns, late.sum())
+    return dict(ev, t=t)
+
+
+def _pushes(ev, sizes, how="host"):
+    ops, a = [], 0
+    for k, n in enumerate(sizes):
+        b = ev["t"].size if n is None else a + n
+        ops.append(("push", how[k % len(how)] if isinstance(how, (list, tuple)) else how, ts_cut(ev, a, b)))
+        a = b
+    assert a == ev["t"].size
+    return ops
+
+
+def _builds(ev, extra=()):
+    t = np.sort(ev["t"])
+    return [("build", int(t[-1]) + 1), ("build", int(t[t.size // 2])), ("build", int(t[t.size // 5]))] + [("build", int(T)) for T in extra]
+
+
+def _s_plain(W, H, how="host", n=30000, seed=11):
+    ev = ts_random_stream(W, H, n, seed)
+    return _pushes(ev, [n // 3, 7, None], how) + _builds(ev)
+
+
+TS_QLEN_PIX = ((3, 2), (5, 2), (7, 2))     # hold qlen - 1, qlen, qlen + 1 events that are not older than TS_QLEN_T
+TS_QLEN_T = 1_030_000_000
+
+
+def _s_qlen(W, H, q):
+    bg = ts_random_stream(W, H, 6000, 21)
+    keep = ~((bg["y"] == 2) & (bg["x"] < 10))
+    bg = {k: v[keep] for k, v in bg.items()}
+    xs, ys, tt = [], [], []
+    for k, (px, py) in enumerate(TS_QLEN_PIX):
+        n_new = q - 1 + k
+        xs += [px] * (2 + n_new); ys += [py] * (2 + n_new)
+        tt += [TS_QLEN_T - 5000 - k, TS_QLEN_T - 1] + [TS_QLEN_T + 700 * j for j in range(n_new)]   # the first new one AT T: not "< T"
+    sp = ts_ev(xs, ys, tt, [(i * 7) % 3 != 0 for i in range(len(xs))])
+    ev = ts_cat(bg, sp)
+    o = np.argsort(ev["t"], kind="stable")
+    ev = {k: v[o] for k, v in ev.items()}
+    return _pushes(ev, [ev["t"].size // 2, None]) + [("build", TS_QLEN_T), ("build", TS_QLEN_T + 1), ("build", int(ev["t"][-1]) + 1)]
+
+
+def _s_t_edges(W, H):
+    ev = ts_random_stream(W, H, 20000, 31)
+    ev["t"][9000:9005] = ev["t"][9004]                                     # five events share one stamp
+    ev["t"][:3] = ev["t"][0]; ev["t"][-3:] = ev["t"][-1]                   # so do the oldest and the newest three
+    t = ev["t"]
+    return [("build", 1_500_000_000)] + _pushes(ev, [12000, None]) + \
+           [("build", int(T)) for T in (t[-1], t[-1] + 1, t[0], t[0] + 1, t[9004], t[9004] + 1)] + [("reset",), ("build", int(t[-1]))]
+
+
+def _s_stamp0_offimage_epoch(W, H):
+    head = ts_ev([5, 6, W, 3, 65535, 6, 9, W - 1], [5, 5, 3, H, 65535, 5, H - 1, 65535], [0, 0, 10, 20, 30, 40, 50, 60], [1, 0, 1, 1, 0, 0, 1, 1])
+    body = ts_random_stream(W, H, 8000, 41, t0=TS_EPOCH, dt=40)            # neighbouring stamps fall on the same double
+    body["x"][1000::997] = W; body["y"][1500::997] = H
+    ev = ts_cat(head, body)
+    t = body["t"]
+    return _pushes(ev, [5, 2000, None]) + [("build", int(T)) for T in (1, 41, 61, t[0], t[4000], t[4000] + 1, t[-1] + 1)]
+
+
+def _s_dev(W, H, kind):
+    ev = ts_random_stream(W, H, 30000, 51)
+    n, t = 30000, ev["t"]
+    if kind in ("dev", "devnopol"):
+        return _pushes(ev, [n // 2, None], kind) + _builds(ev)
+    if kind == "dev-then-host":
+        return _pushes(ev, [n // 2, None], ["dev", "host"]) + _builds(ev, [t[-1]])
+    a, b = ts_cut(ev, 0, 10000), ts_cut(ev, 10000, 20000)                  # dev-drain-then-build
+    return [("push", "dev", a), ("sync",), ("build", int(t[9999]) + 1), ("build", int(t[9999])), ("build", int(t[5000])),
+            ("push", "host", b), ("build", int(t[19999]) + 1), ("build", int(t[19999])),
+            ("push", "dev", ts_cut(ev, 20000, n)), ("build", int(t[-1]) + 1), ("build", int(t[15000]))]
+
+
+def _s_packet(W, H):
+    ev = ts_random_stream(W, H, 4095 + 4096 + 4096 + 5000, 61)
+    return _pushes(ev, [4095, 4096, 4096, None], ["packet", "packet", "packetnopol", "packet"]) + _builds(ev)
+
+
+def _s_unord(W, H, kind):
+    on = [("unordered", 1)]
+    if kind == "ties":            # 50 distinct stamps in random arrival order: ties with the running maximum, the later arrival wins
+        rng = np.random.default_rng(71)
+        n = 3000
+        ev = ts_ev(rng.integers(0, W, n), rng.integers(0, H, n), 1_000_000_000 + 1000 * rng.integers(0, 50, n), rng.integers(0, 2, n))
+        return on + _pushes(ev, [1500, None]) + [("build", 1_000_050_000), ("build", 1_000_049_000), ("build", 1_000_025_000)]
+    if kind == "carry-wins-blocks":   # three whole scan blocks older than the event carried from the first push
+        first = ts_ev([10, 11, 12], [20, 20, 20], [1_000_000_000, 1_900_000_000, 1_000_000_500], [1, 0, 1])
+        older = ts_random_stream(W, H, 3072, 72, t0=1_100_000_000)
+        mixed = ts_random_stream(W, H, 2500, 73, t0=1_899_000_000, dt=1000)   # crosses the carried stamp half-way
+        assert older["t"].max() < 1_900_000_000 < mixed["t"].max() and mixed["t"][800] < 1_900_000_000
+        return on + [("push", "host", first), ("push", "host", older), ("build", 1_900_000_001), ("build", 1_900_000_000),
+                     ("push", "host", mixed), ("build", int(mixed["t"].max()) + 1), ("build", 1_900_000_001)]
+    if kind == "switched-on-late":
+        a = ts_random_stream(W, H, 4000, 74)
+        b = ts_jitter(ts_random_stream(W, H, 4000, 75), 76)
+        return [("push", "host", ts_cut(a, 0, 2000)), ("unordered_refused",), ("push", "host", ts_cut(a, 2000, 4000))] + _builds(a) + \
+               [("reset",), ("unordered", 1)] + _pushes(b, [1000, None]) + _builds(b)
+    ev = ts_jitter(ts_random_stream(W, H, 1024 + 1025 + 2048 + 1 + 1023 + 3000, 77), 78)
+    how = {"sizes": "host", "nopol": "nopol", "dev": ["dev", "devnopol"], "forward": "host"}[kind]
+    return on + _pushes(ev, [1024, 1025, 2048, 1, 1023, None], how) + _builds(ev)
+
+
+def _s_order_flag(W, H):
+    ev = ts_random_stream(W, H, 6000, 81)
+    t_end = int(ev["t"][-1]) + 1
+    a = ts_cut(ev, 0, 1000)
+    bad = ts_cut(ev, 1000, 2000)
+    bad = dict(bad, t=bad["t"].copy()); bad["t"][500] = bad["t"][498] - 1                       # violation inside a push
+    across = ts_cut(ev, 600, 1600)                                                               # ordered in itself, starts before a's end
+    assert across["t"][0] < a["t"][-1]
+    later = ts_cut(ev, 2000, 3000)
+    fresh = ts_cut(ev, 3000, 6000)
+    return [("push", "host", a), ("build", t_end), ("push", "host", bad), ("refused", t_end, TS_UNSUPPORTED), ("reset",),
+            ("push", "host", a), ("push", "host", across), ("refused", t_end, TS_UNSUPPORTED),
+            ("push", "host", later), ("refused", t_end, TS_UNSUPPORTED),                         # sticky over ordered pushes
+            ("reset",), ("push", "host", fresh), ("build", t_end), ("build", int(fresh["t"][1500])), ("fresh", fresh, int(fresh["t"][1500]))]
+
+
+TS_FWD_BLOCKS = (((20, 20, 10, 10), (100.5, 50.5), 0), ((40, 20, 6, 6), (120.25, 50.75), 1), ((60, 20, 4, 8), (140.5, 60.5), None))
+TS_FWD_EXTRA = ((70, 20), (139.5, 60.5))   # one more source next to the 4 x 8 block's point: 33 contributions on two of its pixels
+
+
+def ts_handbuilt_lut(W, H):
+    """Raw pixel -> rectified point table with whole source blocks sent to one point (x0, y0, w, h) -> (u, v): 100, 36 (> the fold
+    kernel's 32-entry register list) and exactly 32 contributions per destination, 33 where TS_FWD_EXTRA overlaps; every rejection of
+    TimeSurface.cpp:90,95 on the first row; NaN (no contribution) above row 100 elsewhere, a quarter-pixel shift below."""
+    lut = np.full((H, W, 2), np.nan)
+    yy, xx = np.mgrid[100:H, 0:W]
+    lut[100:, :, 0] = xx + 0.25; lut[100:, :, 1] = yy - 0.5
+    for (x0, y0, w, h), uv, _ in TS_FWD_BLOCKS:
+        lut[y0:y0 + h, x0:x0 + w] = uv
+    lut[TS_FWD_EXTRA[0][1], TS_FWD_EXTRA[0][0]] = TS_FWD_EXTRA[1]
+    for x, uv in enumerate(((np.nan, 10), (-0.5, 10), (W - 1, 10), (W - 1.5, 10), (W, 10), (10, H - 1), (10, H - 1.5), (10, np.nan), (12, -0.25),
+                            (0.0, 0.0), (W - 2.0, H - 2.0))):
+        lut[0, x] = uv
+    return lut
+
+
+def _s_fwd_handbuilt(W, H):
+    rng = np.random.default_rng(91)
+    xs, ys, ps = [], [], []
+    for (x0, y0, w, h), _, pol in TS_FWD_BLOCKS:
+        for y in range(y0, y0 + h):
+            for x in range(x0, x0 + w):
+                xs.append(x); ys.append(y); ps.append(int(rng.integers(0, 2)) if pol is None else pol)
+    xs.append(TS_FWD_EXTRA[0][0]); ys.append(TS_FWD_EXTRA[0][1]); ps.append(1)
+    xs += list(range(11)); ys += [0] * 11; ps += [1, 0] * 5 + [1]
+    o = rng.permutation(len(xs))                                           # arrival order is not raster order
+    sp = ts_ev(np.array(xs)[o], np.array(ys)[o], np.zeros(len(xs)), np.array(ps)[o])
+    bg = ts_random_stream(W, H, 12000, 92)
+    bg["y"][:] = np.maximum(bg["y"], 30)                                   # keeps the first row and the blocks to the hand-placed events
+    ev = ts_cat(bg, sp)
+    ev["t"][bg["t"].size:] = bg["t"][-1] + 1 + np.arange(len(xs)) * 50     # newest: decay close to 1, |sum| far beyond 1
+    return _pushes(ev, [5000, None]) + [("build", int(ev["t"][-1]) + 1), ("build", int(ev["t"][-40])), ("build", int(ev["t"][-1]) + 1)]
+
+
+def _s_evict(W, H):
+    """Five pushes of 1.5 M events into the 4 Mi log: folds at the third and at the fifth push (back on the first buffer set)."""
+    rng = np.random.default_rng(5)
+    n_batch, ops, tt = 1_500_000, [], []
+    for b in range(5):
+        x = rng.integers(0, W, n_batch); y = rng.integers(0, H, n_batch)
+        if b > 0:
+            x[x < 40] += 40                                                # these pixels' values come from the base grids
+        t = 1_000_000_000 + (b * n_batch + np.arange(n_batch)) * 40
+        tt.append(t)
+        ops.append(("push", "host", ts_ev(x, y, t, rng.integers(0, 2, n_batch))))
+    t = np.concatenate(tt)
+    r0 = t.size - (n_batch + TS_LOG_CAP // 4)                              # first resident event after the second fold
+    big = ts_ev(np.zeros(TS_LOG_CAP // 2 + 1), np.zeros(TS_LOG_CAP // 2 + 1), np.full(TS_LOG_CAP // 2 + 1, int(t[-1]) + 5))
+    return ops + [("build", int(t[-1]) + 1000), ("build", int(t[-200_000])), ("build", int(t[r0 + 1])), ("build", int(t[r0])),
+                  ("build", int(t[r0 - 1]) + 1), ("refused", int(t[r0 - 1]), TS_UNSUPPORTED), ("refused", int(t[r0 - 21]), TS_UNSUPPORTED),
+                  ("refused", int(t[2_000_000]), TS_UNSUPPORTED), ("refused", int(t[0]), TS_UNSUPPORTED),
+                  ("push_refused", big, TS_CAPACITY), ("build", int(t[-1]) + 1000)]
+
+
+def _sc(id, script, size="hkust", cams=(0, 1), lut=None, **prm):
+    return dict(id=id, size=size, prm=prm, script=script, cams=cams, lut=lut)
+
+
+FWD = dict(time_surface_mode=1)
+TS_CASES = [
+    _sc("bwd-median0", _s_plain, median_blur_kernel_size=0),
+    _sc("bwd-median0-pol", _s_plain, median_blur_kernel_size=0, ignore_polarity=0),
+    _sc("median2-refused", lambda W, H: [("push", "host", ts_random_stream(W, H, 3000, 12)), ("refused", 2_000_000_000, TS_UNSUPPORTED), ("sync",),
+                                         ("refused", 1_003_000_000, TS_UNSUPPORTED), ("reset",), ("push", "host", ts_random_stream(W, H, 3000, 13))],
+        median_blur_kernel_size=2),
+    _sc("decay-1ms", _s_plain, decay_ms=1.0),
+    _sc("decay-1s", _s_plain, decay_ms=1000.0, ignore_polarity=0),
+    _sc("qlen-1", lambda W, H: _s_qlen(W, H, 1), max_event_queue_len=1),
+    _sc("qlen-2", lambda W, H: _s_qlen(W, H, 2), max_event_queue_len=2),
+    _sc("qlen-64", lambda W, H: _s_qlen(W, H, 64), max_event_queue_len=64),
+    _sc("t-edges", _s_t_edges),
+    _sc("stamp0-offimage-epoch", _s_stamp0_offimage_epoch, ignore_polarity=0),
+    _sc("stamp0-offimage-epoch-fwd", _s_stamp0_offimage_epoch, **FWD),
+    _sc("dev-push", lambda W, H: _s_dev(W, H, "dev")),
+    _sc("dev-push-nopol", lambda W, H: _s_dev(W, H, "devnopol"), ignore_polarity=0),
+    _sc("dev-then-host", lambda W, H: _s_dev(W, H, "dev-then-host")),
+    _sc("dev-drain-then-build", lambda W, H: _s_dev(W, H, "dev-drain-then-build")),
+    _sc("dev-push-fwd", lambda W, H: _s_dev(W, H, "dev"), **FWD),
+    _sc("packet-4095-4096", _s_packet, ignore_polarity=0),
+    _sc("unord-ties", lambda W, H: _s_unord(W, H, "ties"), ignore_polarity=0),
+    _sc("unord-carry-wins-blocks", lambda W, H: _s_unord(W, H, "carry-wins-blocks"), ignore_polarity=0),
+    _sc("unord-1024-1025-2048", lambda W, H: _s_unord(W, H, "sizes"), ignore_polarity=0),
+    _sc("unord-nopol", lambda W, H: _s_unord(W, H, "nopol"), ignore_polarity=0),
+    _sc("unord-dev", lambda W, H: _s_unord(W, H, "dev"), ignore_polarity=0),
+    _sc("unord-forward", lambda W, H: _s_unord(W, H, "forward"), ignore_polarity=0, **FWD),
+    _sc("unord-switched-on-late", lambda W, H: _s_unord(W, H, "switched-on-late")),
+    _sc("order-flag", _s_order_flag),
+    _sc("order-flag-fwd", _s_order_flag, **FWD),
+    _sc("fwd-handbuilt", _s_fwd_handbuilt, lut=ts_handbuilt_lut, ignore_polarity=0, median_blur_kernel_size=0, **FWD),
+    _sc("fwd-handbuilt-median", _s_fwd_handbuilt, lut=ts_handbuilt_lut, ignore_polarity=1, **FWD),
+    _sc("size-small", lambda W, H: _s_plain(W, H, n=8000), size="small"),
+    _sc("size-small-fwd", lambda W, H: _s_plain(W, H, n=8000), size="small", ignore_polarity=0, **FWD),
+    _sc("size-odd", lambda W, H: _s_plain(W, H, n=20000), size="odd", ignore_polarity=0),
+    _sc("size-odd-fwd", lambda W, H: _s_plain(W, H, n=20000), size="odd", **FWD),
+    _sc("size-dsec-median0", lambda W, H: _s_plain(W, H, n=40000), size="dsec", median_blur_kernel_size=0),
+    _sc("evict-T-before-resident", _s_evict, cams=(0,)),
+]
+TS_CASES = {c["id"]: c for c in TS_CASES}
+
+
+def ts_case_script(c):
+    W, H = TS_SIZES[c["size"]]
+    return c["script"](W, H)
+
+
+def ts_case_params(c, lib):
+    p = configs.params_for("dsec" if c["size"] == "dsec" else "hkust", lib)
+    for k, v in c["prm"].items():
+        setattr(p, k, v)
+    return p
+
+
+def ts_effective(ops):
+    """What the reference's eventsCallback queues for the pushes of a script, one stream per segment between resets
+    (tests/indep_numpy.py::events_callback_queue; a stream whose stamps never decrease is its own answer: every insertion stops at
+    once and back() is the new event)."""
+    import indep_numpy as ind
+    seg = [[]]
+    for op in ops:
+        if op[0] == "push":
+            seg[-1].append(dict(op[2], p=np.ones_like(op[2]["p"])) if "nopol" in op[1] else op[2])     # pol = NULL queues polarity 1
+        elif op[0] == "reset":
+            seg.append([])
+    out = []
+    for s in seg:
+        ev = ts_cat(*s) if s else ts_ev([], [], [])
+        out.append(ev if np.all(np.diff(ev["t"]) >= 0) else ind.events_callback_queue(ev))
+    return out
+
+
+def ts_host_model(ops):
+    """The host-side bookkeeping of ts_push / ts_run_build / drain (host_knows, host_max_t, log folds) replayed over a script: which
+    branch every push and build takes, as a list of sets of tags, one per op."""
+    knows, hmax, stamps, unordered, dev_seen, tags = True, None, [], False, False, []
+    log_n, folds, fold_t = 0, 0, None
+    eff = ts_effective(ops)
+    seg, pushed = 0, 0
+    for op in ops:
+        tg = set()
+        if op[0] == "push":
+            ev, how = op[2], op[1]
+            n = ev["t"].size
+            if log_n + n > TS_LOG_CAP:
+                keep = min(log_n, TS_LOG_CAP // 4)
+                fold_t = int(eff[seg]["t"][pushed - keep - 1]); log_n = keep; folds += 1
+                tg.add("fold%d" % folds)
+            run_max = int(eff[seg]["t"][pushed - 1]) if pushed else None
+            dev = how.startswith("dev")
+            tg.add(how)
+            if unordered:
+                tg.add("unordered")
+                if pushed == 0:
+                    tg.add("scan-empty-carry")
+                for b in range(0, n, 1024):
+                    blk = ev["t"][b:b + 1024]
+                    if run_max is not None and blk.max() < run_max:
+                        tg.add("scan-block-older-than-carry")
+                    if run_max is not None and b == 0 and blk[0] == run_max:
+                        tg.add("scan-tie-with-carry")
+                inc = np.maximum.accumulate(ev["t"])
+                if np.any(ev["t"][1:] == inc[:-1]):
+                    tg.add("scan-tie")
+                tg.add("scan-n%d" % n)
+            if dev or unordered:
+                knows = False
+            elif knows:
+                if hmax is None or ev["t"][-1] >= hmax:
+                    hmax = int(ev["t"][-1])
+                else:
+                    knows = False
+            if not dev and dev_seen:
+                tg.add("host-after-dev")
+            dev_seen |= dev
+            if how.startswith("packet"):
+                tg.add("packet-one-copy" if (how == "packet" and n >= 4096) else "packet-four-copies")
+            if not unordered:
+                if np.any(np.diff(ev["t"]) < 0):
+                    tg.add("order-violation-inside")
+                elif run_max is not None and ev["t"][0] < run_max:
+                    tg.add("order-violation-across")
+            pushed += n; log_n += n
+            stamps = eff[seg]["t"][:pushed]
+        elif op[0] == "sync":
+            if not knows and not unordered:
+                knows, hmax = True, (int(stamps.max()) if len(stamps) else None)
+                tg.add("drain-refreshes-host")
+        elif op[0] == "reset":
+            knows, hmax, stamps, dev_seen, log_n, fold_t = True, None, [], False, 0, None
+            seg += 1; pushed = 0
+        elif op[0] == "unordered":
+            unordered = bool(op[1])
+        elif op[0] in ("build", "refused"):
+            T = op[1]
+            if log_n == 0:
+                tg.add("empty-log")
+            fast = knows and (log_n == 0 or T > hmax)
+            general = len(stamps) > 0 and T <= int(stamps[-1])
+            tg.add("fast" if fast else ("general" if general else "general-launched-as-no-op"))
+            assert not (fast and general)
+            if knows and hmax is not None and T == hmax:
+                tg.add("T==host_max_t")
+            if knows and hmax is not None and T == hmax + 1:
+                tg.add("T==host_max_t+1")
+            if len(stamps) and T == int(stamps[0]):
+                tg.add("T==oldest")
+            if len(stamps) and np.sum(stamps == T) >= 3:
+                tg.add("T==shared-stamp")
+            if fold_t is not None:
+                tg.add("T<=folded" if T <= fold_t else "T>folded")
+                if T == int(stamps[pushed - log_n]):
+                    tg.add("T==oldest-resident")
+        tags.append(tg)
+    return tags
