@@ -1,10 +1,10 @@
 """Calibration and parameter sets of the reference's shipped datasets (values only).
 
 Sources (all under /root/reference/esvo_core/):
-  calib/hkust/{left,right}.yaml, calib/dsec/zurich_city_04_a/{left,right}.yaml,
-  cfg/mapping/mapping_{hkust,dsec}.yaml, cfg/tracking/tracking_{hkust,dsec}.yaml,
+  calib/hkust/{left,right}.yaml, calib/dsec/zurich_city_04_a/{left,right}.yaml, calib/rpg/{left,right}.yaml,
+  cfg/mapping/mapping_{hkust,dsec}.yaml, cfg/tracking/tracking_{hkust,dsec}.yaml, cfg/mvstereo/mvstereo_{rpg,upenn}.yaml,
   ../esvo_time_surface/cfg/parameters.yaml.
-"A" = 346x260 (hkust DAVIS346), "B" = 640x480 (DSEC-shaped).
+"A" = 346x260 (hkust DAVIS346), "B" = 640x480 (DSEC-shaped), rpg = 240x180 (DAVIS240C).
 """
 from __future__ import annotations
 
@@ -58,7 +58,88 @@ RIGS = {
                -7.83382948021244e-07, 0.0050068717705076754, 0.9999874655386736],
             P=[199.6530123165822, 0.0, 177.43276376280926, -19.941771812941038, 0.0, 199.6530123165822, 126.81215684365904, 0.0,
                0.0, 0.0, 1.0, 0.0])),
+    # calib/rpg/{left,right}.yaml -- the stereo DAVIS240C rig of the rpg datasets (esvo_MVStereo's mvstereo_rpg.launch)
+    "rpg": dict(
+        width=240, height=180, model="plumb_bob",
+        left=dict(
+            K=[196.639, 0, 105.064, 0, 196.733, 72.4717, 0.0, 0.0, 1.0],
+            D=[-0.336733, 0.111789, -0.00140053, -0.000459594],
+            R=[0.999791, -0.018779, -0.00802416, 0.0187767, 0.999824, -0.000360707, 0.00802952, 0.000209964, 0.999968],
+            P=[156.925, 0, 108.167, 0, 0, 156.925, 78.4205, 0, 0, 0, 1, 0]),
+        right=dict(
+            K=[196.426, 0, 110.745, 0, 196.564, 88.1131, 0.0, 0.0, 1.0],
+            D=[-0.346294, 0.12772, -0.000272051, -0.000195801],
+            R=[0.999589, 0.0222217, -0.0181009, -0.0222166, 0.999753, 0.000486491, 0.0181073, -8.41512e-05, 0.999836],
+            P=[156.925, 0, 108.167, -23.2327, 0, 156.925, 78.4205, 0, 0, 0, 1, 0])),
 }
+
+# cfg/mvstereo/mvstereo_{rpg,upenn}.yaml: the keys of the esvo_MVStereo node (the loop's own keys first, then the
+# mapping back-end's).  Values only.  MVStereoMode: 0 PURE_EVENT_MATCHING, 1 PURE_BLOCK_MATCHING, 2 EM_PLUS_ESTIMATION,
+# 3 BM_PLUS_ESTIMATION (ESVO's mapper), 4 PURE_SEMI_GLOBAL_MATCHING.  dvs_frame_id comes from the launch file: the rpg
+# ground truth is the marker's pose ("marker"), the upenn one the left camera's ("dvs").
+MVSTEREO = {k: dict(rpg=a, upenn=b) for k, a, b in [
+    #  key                           rpg         upenn
+        ("MVStereoMode",              3,          3),
+        ("EM_Slice_Thickness",        0.001,      0.001),
+        ("EM_Time_THRESHOLD",         0.0005,     0.0005),
+        ("EM_EPIPOLAR_THRESHOLD",     1.0,        1.0),
+        ("EM_TS_NCC_THRESHOLD",       0.1,        0.1),
+        ("EM_NUM_EVENT_MATCHING",     3000,       3000),
+        ("BM_half_slice_thickness",   0.001,      0.001),
+        ("PROCESS_EVENT_NUM",         1000,       1000),
+        ("TS_HISTORY_LENGTH",         100,        100),
+        ("mapping_rate_hz",           20,         20),
+        ("Denoising",                 True,       False),
+        ("dvs_frame_id",              "marker",   "dvs"),
+        ("invDepth_min_range",        0.2,        0.16),
+        ("invDepth_max_range",        2.0,        1.0),
+        ("residual_vis_threshold",    20,         20),
+        ("stdVar_vis_threshold",      0.015,      0.15),
+        ("age_vis_threshold",         1,          1),
+        ("fusion_radius",             0,          0),
+        ("FUSION_STRATEGY",           "CONST_FRAMES", "CONST_POINTS"),
+        ("maxNumFusionFrames",        40,         40),
+        ("maxNumFusionPoints",        5000,       3000),
+        ("SmoothTimeSurface",         False,      False),
+        ("Regularization",            True,       False),
+        ("patch_size_X",              15,         15),
+        ("patch_size_Y",              7,          7),
+        ("Tdist_nu",                  2.1897,     2.182),
+        ("Tdist_scale",               16.6397,    17.277),
+        ("BM_min_disparity",          1,          1),
+        ("BM_max_disparity",          40,         40),
+        ("BM_step",                   1,          1),
+        ("BM_ZNCC_Threshold",         0.1,        0.1),
+        ("BM_bUpDownConfiguration",   False,      False),
+]}
+
+
+def mvstereo_config(name):
+    """The MVSTEREO column of one dataset as a dict."""
+    return {k: v[name] for k, v in MVSTEREO.items()}
+
+
+def mvstereo_params_for(name, lib) -> capi.Params:
+    """esvo_params of the esvo_MVStereo node with cfg/mvstereo/mvstereo_<name>.yaml (time surfaces: the ts parameters; the
+    node's ITERATION_OPTIMIZATION and regularisation radius / neighbours keep their constructor defaults 10 / 5 / 8 / 8)."""
+    c = mvstereo_config(name)
+    p = capi.default_params(lib)
+    p.decay_ms = 30.0; p.ignore_polarity = 1; p.median_blur_kernel_size = 1
+    p.max_event_queue_len = 20; p.time_surface_mode = 0
+    p.patch_size_x, p.patch_size_y = c["patch_size_X"], c["patch_size_Y"]
+    p.bm_step = c["BM_step"]; p.bm_zncc_threshold = c["BM_ZNCC_Threshold"]; p.bm_updown = int(c["BM_bUpDownConfiguration"])
+    p.bm_min_disparity, p.bm_max_disparity = c["BM_min_disparity"], c["BM_max_disparity"]
+    p.lsnorm = capi.LSNORM_TDIST; p.max_iteration = 10
+    p.td_nu, p.td_scale = c["Tdist_nu"], c["Tdist_scale"]
+    p.invdepth_min_range, p.invdepth_max_range = c["invDepth_min_range"], c["invDepth_max_range"]
+    p.residual_vis_threshold = c["residual_vis_threshold"]; p.stdvar_vis_threshold = c["stdVar_vis_threshold"]
+    p.age_vis_threshold = c["age_vis_threshold"]; p.fusion_radius = c["fusion_radius"]
+    p.fusion_strategy = capi.FUSION_CONST_FRAMES if c["FUSION_STRATEGY"] == "CONST_FRAMES" else capi.FUSION_CONST_POINTS
+    p.max_num_fusion_frames = c["maxNumFusionFrames"]; p.max_num_fusion_points = c["maxNumFusionPoints"]
+    p.smooth_time_surface = int(c["SmoothTimeSurface"]); p.regularization = int(c["Regularization"])
+    p.reg_radius, p.reg_min_neighbours, p.reg_min_close_neighbours = 5, 8, 8
+    p.num_thread_mapping = 4
+    return p
 
 
 def rig_calibs(name):

@@ -10,12 +10,20 @@ import numpy as np
 from .configs import rig_arrays
 
 
-def _rect_to_raw(cam, uv):
-    """Rectified pixel (sub-pixel) -> raw pixel: same math as initUndistortRectifyMap (plumb_bob)."""
+def _rect_to_raw(cam, uv, equidistant=False):
+    """Rectified pixel (sub-pixel) -> raw pixel: same math as initUndistortRectifyMap (plumb_bob, or with equidistant=True
+    cv::fisheye::initUndistortRectifyMap)."""
     K, D, R, P = cam["K"], cam["D"], cam["R"], cam["P"]
     iR = np.linalg.inv(P[:, :3] @ R)
     h = np.concatenate([uv, np.ones((uv.shape[0], 1))], axis=1) @ iR.T
     x = h[:, 0] / h[:, 2]; y = h[:, 1] / h[:, 2]
+    if equidistant:
+        r = np.sqrt(x * x + y * y)
+        th = np.arctan(r)
+        th2 = th * th
+        thd = th * (1 + th2 * (D[0] + th2 * (D[1] + th2 * (D[2] + th2 * D[3]))))
+        s = np.where(r > 0, thd / np.maximum(r, 1e-300), 1.0)
+        return np.stack([K[0, 0] * x * s + K[0, 2], K[1, 1] * y * s + K[1, 2]], axis=1)
     r2 = x * x + y * y
     kr = 1 + (D[1] * r2 + D[0]) * r2
     xd = x * kr + 2 * D[2] * x * y + D[3] * (r2 + 2 * x * x)
@@ -38,10 +46,12 @@ def pose_at(t, amp=0.05, rot_deg=2.0, period=1.0):
 
 def make_stream(rig="hkust", seed=2, t_ts=0.5, history_ms=60.0, n_segments=80, depth_range=None,
                 n_seeds=5000, bm_window_ms=10.0, pose_dt_us=50.0, noise_frac=0.02, speed=1.0,
-                sample_hz=1000.0):
+                sample_hz=1000.0, translation_scale=None, rig_model=False):
     """Returns a dict with left/right raw event arrays (sorted by time), the TS stamp, the seed
     events (newest first, as esvo_Mapping::dataTransferring gathers them, esvo_Mapping.cpp:562-575),
-    the sampled virtual-view poses (:585-599) and the scene points."""
+    the sampled virtual-view poses (:585-599) and the scene points.  translation_scale: the factor on the trajectory's
+    translation (default 1 on hkust, 20 elsewhere); rig_model=True distorts with the rig's own model (equidistant on upenn)
+    instead of plumb_bob everywhere."""
     cams = rig_arrays(rig)
     W, H = cams["width"], cams["height"]
     rng = np.random.default_rng(seed)
@@ -60,7 +70,9 @@ def make_stream(rig="hkust", seed=2, t_ts=0.5, history_ms=60.0, n_segments=80, d
         a = np.array([(u0 - cx) * z0 / f, (v0 - cy) * z0 / f, z0]); b = np.array([(u1 - cx) * z1 / f, (v1 - cy) * z1 / f, z1])
         pts.append(a * (1 - s) + b * s)
     pts = np.concatenate(pts, axis=0)
-    scale_t = 1.0 if rig == "hkust" else 20.0  # translate more in the large-scale scene
+    scale_t = (1.0 if rig == "hkust" else 20.0) if translation_scale is None else translation_scale  # translate more in the large-scale scene
+    from .configs import RIGS
+    equidistant = rig_model and RIGS[rig]["model"] == "equidistant"
 
     def project(t):
         T = pose_at(t * speed); T[:3, 3] *= scale_t
@@ -71,7 +83,7 @@ def make_stream(rig="hkust", seed=2, t_ts=0.5, history_ms=60.0, n_segments=80, d
             P = cams[side]["P"]
             hom = pc @ P[:, :3].T + P[:, 3]
             uv = hom[:, :2] / hom[:, 2:3]
-            raw = _rect_to_raw(cams[side], uv)
+            raw = _rect_to_raw(cams[side], uv, equidistant)
             ok = (pc[:, 2] > 0.1) & (raw[:, 0] >= 0) & (raw[:, 0] < W) & (raw[:, 1] >= 0) & (raw[:, 1] < H)
             out.append((np.floor(raw).astype(np.int64), ok))
         return out, T

@@ -499,7 +499,107 @@ inline void eventSlicingForEM(std::vector<esvo::Event*>& vEventsPtr_left, int64_
     if (it_tmp == vEventsPtr_left.end()) break;
   }
 }
+//  * selectEMEvents: the event-matching branch of esvo_MVStereo::dataTransferring (esvo_MVStereo.cpp:579-609), one event
+//    queue at a time.  The window is [lower_bound(t_low), lower_bound(t_up) - 1): the walk stops one event short of
+//    lower_bound(t_up), and `<=` on the count lets EM_numEventMatching + 1 events through.  Returns false where the
+//    reference returns "no events": lower_bound(t_low) == lower_bound(t_up) - 1.  With no event at all in [t_low, t_up)
+//    the reference decrements past lower_bound(t_low) (or past begin()) and walks out of the window (undefined); that case
+//    is answered the same way, false and nothing selected.
+template <class EventBuffer>
+inline bool selectEMEvents(EventBuffer& events, int64_t t_low_ns, int64_t t_up_ns, size_t EM_numEventMatching,
+                           std::vector<esvo::Event*>& vEventsPtr) {
+  vEventsPtr.clear();
+  auto lower = [&](int64_t t) {   // tools::EventBuffer_lower_bound (utils.h:50-55): toSec() doubles
+    const double ts = toSec(t);
+    size_t lo = 0, hi = events.size();
+    while (lo < hi) { size_t mid = (lo + hi) / 2; if (toSec(events[mid].ts) < ts) lo = mid + 1; else hi = mid; }
+    return lo;
+  };
+  size_t lo = lower(t_low_ns);
+  const size_t up = lower(t_up_ns);
+  if (up <= lo + 1) return false;
+  while (lo != up - 1 && vEventsPtr.size() <= EM_numEventMatching) vEventsPtr.push_back(&events[lo++]);
+  return true;
+}
 }  // namespace frontend
+}  // namespace esvo_core
+
+namespace esvo {
+// The tf::Transformer(true, ros::Duration(100.0)) the nodes keep (esvo_Mapping.cpp:140, esvo_Tracking.cpp:58,
+// esvo_MVStereo.cpp:142), filled by stampedPoseCallback and read by getPoseAt.  Restates the tf2 TimeCache behaviour the
+// nodes rely on (DESIGN.md section 2):
+//  * the pose travels as quaternion + position (PoseStamped) and comes back as a 4x4: q = Eigen::Quaterniond(R) on the way
+//    in, R = q.toRotationMatrix() on the way out -- an exact stamp returns the stored pose after that round trip;
+//  * between two stamps: translation (1 - r) p0 + r p1, rotation tf2 slerp (shortest path), r = (t - t0) / (t1 - t0) in
+//    seconds of ros::Duration;
+//  * no extrapolation: before the oldest or after the newest stamp there is no pose; one entry answers only at its stamp;
+//    stamp 0 means "the latest";
+//  * entries older than the newest minus the cache time (100 s) are dropped; a second pose for a stored stamp is refused.
+class PoseBuffer {
+ public:
+  explicit PoseBuffer(int64_t cache_ns = 100000000000LL) : cache_ns_(cache_ns) {}
+  bool setTransform(int64_t stamp_ns, const Pose& T_world_dvs) {
+    if (!s_.empty() && s_.back().t > stamp_ns + cache_ns_) return false;
+    auto it = std::lower_bound(s_.begin(), s_.end(), stamp_ns, [](const Entry& e, int64_t t) { return e.t < t; });
+    if (it != s_.end() && it->t == stamp_ns) return false;
+    Entry e;
+    e.t = stamp_ns;
+    const double R[9] = {T_world_dvs[0], T_world_dvs[1], T_world_dvs[2], T_world_dvs[4], T_world_dvs[5], T_world_dvs[6],
+                         T_world_dvs[8], T_world_dvs[9], T_world_dvs[10]};
+    quaternionFromRotation(R, e.q);
+    e.p[0] = T_world_dvs[3]; e.p[1] = T_world_dvs[7]; e.p[2] = T_world_dvs[11];
+    s_.insert(it, e);
+    while (s_.front().t + cache_ns_ < s_.back().t) s_.erase(s_.begin());
+    return true;
+  }
+  bool canTransform(int64_t t_ns) const { Pose T; return lookup(t_ns, T); }
+  bool lookup(int64_t t_ns, Pose& T) const {
+    if (s_.empty()) return false;
+    if (t_ns == 0) return toPose(s_.back().q, s_.back().p, T);
+    if (t_ns < s_.front().t || t_ns > s_.back().t) return false;
+    auto it = std::upper_bound(s_.begin(), s_.end(), t_ns, [](int64_t t, const Entry& e) { return t < e.t; });
+    const Entry& a = *(it - 1);
+    if (a.t == t_ns) return toPose(a.q, a.p, T);
+    const Entry& b = *it;
+    const double r = esvo_core::frontend::toSec(t_ns - a.t) / esvo_core::frontend::toSec(b.t - a.t);   // ros::Duration::toSec()
+    double q[4], p[3];
+    for (int i = 0; i < 3; ++i) p[i] = (1.0 - r) * a.p[i] + r * b.p[i];
+    slerp(a.q, b.q, r, q);
+    return toPose(q, p, T);
+  }
+  // tf's getLatestCommonTime for the one world -> dvs link: the newest stamp; false (t untouched) when the buffer is empty
+  bool latestCommonTime(int64_t& t_ns) const {
+    if (s_.empty()) return false;
+    t_ns = s_.back().t;
+    return true;
+  }
+  size_t size() const { return s_.size(); }
+  void clear() { s_.clear(); }
+  // tf2::Quaternion::slerp / angleShortestPath (tf2Acos clamps to [-1, 1]); q = x, y, z, w
+  static void slerp(const double a[4], const double b[4], double t, double out[4]) {
+    auto dot = [](const double* u, const double* v) { return u[0] * v[0] + u[1] * v[1] + u[2] * v[2] + u[3] * v[3]; };
+    const double s = std::sqrt(dot(a, a) * dot(b, b)), d_ab = dot(a, b);
+    const double c = std::max(-1.0, std::min(1.0, (d_ab < 0 ? -d_ab : d_ab) / s));
+    const double theta = std::acos(c) * 2.0 / 2.0;
+    if (theta == 0.0) { std::copy(a, a + 4, out); return; }
+    const double d = 1.0 / std::sin(theta), s0 = std::sin((1.0 - t) * theta), s1 = std::sin(t * theta);
+    const double sg = d_ab < 0 ? -1.0 : 1.0;
+    for (int i = 0; i < 4; ++i) out[i] = (a[i] * s0 + sg * b[i] * s1) * d;
+  }
+ private:
+  struct Entry { int64_t t; double q[4]; double p[3]; };
+  static bool toPose(const double q[4], const double p[3], Pose& T) {
+    double R[9];
+    rotationFromQuaternion(q, R);
+    T = {R[0], R[1], R[2], p[0], R[3], R[4], R[5], p[1], R[6], R[7], R[8], p[2], 0, 0, 0, 1};
+    return true;
+  }
+  int64_t cache_ns_;
+  std::vector<Entry> s_;   // oldest first
+};
+}  // namespace esvo
+
+namespace esvo_core {
 
 // esvo_core::esvo_Mapping::MappingAtTime (esvo_Mapping.cpp:261-399) as one call with device-resident hand-off.
 class esvo_Mapping {
@@ -693,6 +793,187 @@ class esvo_Mapping {
   PoseProvider getPoseAt_;
 };
 
+// The host half of the esvo_MVStereo node (esvo_MVStereo.cpp:179-237,552-880,1002-1039): the event queues, the
+// time-surface history, the tf pose buffer fed by the stamped_pose topic, the three reset rules, getPoseAt, the per-mode
+// dataTransferring windows and the BM denoising step of MappingAtTime.  Host logic only -- no device call, so it builds
+// and is tested without the library; esvo_MVStereo below owns one and runs MappingAtTime on what it selects.
+// Modes use esvo_MVStereo::eMVStereoMode numbering (0 EM, 1 BM, 2 EM + estimation, 3 BM + estimation, 4 SGM).
+class MVStereoFrontEnd {
+ public:
+  MVStereoFrontEnd(int width, int height, int msm) : W_((size_t)width), H_((size_t)height), msm_(msm) {}
+  // node parameters (constructor defaults of esvo_MVStereo.cpp:71-101; cfg/mvstereo/*.yaml override them)
+  size_t PROCESS_EVENT_NUM_ = 500, TS_HISTORY_LENGTH_ = 100, EM_numEventMatching_ = 3000;
+  double BM_half_slice_thickness_ = 0.001;
+  bool bDenoising_ = false;
+  bool marker_frame_ = false;   // dvs_frame_id "marker" (mvstereo_rpg.launch): getPoseAt appends T_marker_cam
+  static constexpr size_t MAX_NUM_Event_INVOLVED = 10000;   // BM window cap (:639)
+
+  // ---- callbacks.  Each returns true when its reset rule fired: reset() ran before the new data was added. ----
+  // eventsCallback (:746-780): dt = first new stamp - newest queued stamp of the same queue; dt < 0 or >= 0.5 s resets.
+  // Then insertion-sorted, capped at 3e6.  (The reference reads events[0] before its emptiness check; an empty packet
+  // here changes nothing.)
+  bool eventsCallback(const std::vector<esvo::Event>& events, bool left) {
+    if (events.empty()) return false;
+    bool was_reset = false;
+    std::deque<esvo::Event>* EQ = left ? &events_left_ : &events_right_;
+    if (!EQ->empty() && inconsistent(events[0].ts, EQ->back().ts)) { reset(); was_reset = true; }
+    for (const esvo::Event& e : events) {
+      EQ->push_back(e);
+      long i = (long)EQ->size() - 2;
+      while (i >= 0 && (*EQ)[(size_t)i].ts > e.ts) { (*EQ)[(size_t)i + 1] = (*EQ)[(size_t)i]; --i; }
+      (*EQ)[(size_t)(i + 1)] = e;
+    }
+    static constexpr size_t MAX_EVENT_QUEUE_LENGTH = 3000000;   // clearEventQueue (:782-790)
+    if (EQ->size() > MAX_EVENT_QUEUE_LENGTH) EQ->erase(EQ->begin(), EQ->begin() + (long)(EQ->size() - MAX_EVENT_QUEUE_LENGTH));
+    return was_reset;
+  }
+  // timeSurfaceCallback (:792-838): dt against the newest stamp in TS_history_; dt < 0 or >= 0.5 s resets.  The pair is
+  // emplaced (a stamp already present keeps its old images), TS_id_ counts every call, the history keeps TS_HISTORY_LENGTH.
+  bool timeSurfaceCallback(int64_t stamp_ns, const uint8_t* time_surface_left, const uint8_t* time_surface_right) {
+    bool was_reset = false;
+    if (!TS_history_.empty() && inconsistent(stamp_ns, TS_history_.rbegin()->first)) { reset(); was_reset = true; }
+    const size_t n = W_ * H_;
+    TS_history_.emplace(stamp_ns, TsPair{std::vector<uint8_t>(time_surface_left, time_surface_left + n),
+                                         std::vector<uint8_t>(time_surface_right, time_surface_right + n), TS_id_});
+    ++TS_id_;
+    while (TS_history_.size() > TS_HISTORY_LENGTH_) TS_history_.erase(TS_history_.begin());
+    return was_reset;
+  }
+  // stampedPoseCallback (:670-706): tf's latest common time is read first (tf2 writes it only on success, so after a
+  // reset emptied the buffer the previous value stays); when it is not 0, dt = new stamp - it, and dt < 0 or >= 0.5 s
+  // resets.  Then the pose goes into tf.
+  bool stampedPoseCallback(int64_t stamp_ns, const esvo::Pose& T_world_dvs) {
+    bool was_reset = false;
+    tf_.latestCommonTime(tf_latest_common_time_);
+    if (frontend::toSec(tf_latest_common_time_) != 0 && inconsistent(stamp_ns, tf_latest_common_time_)) { reset(); was_reset = true; }
+    tf_.setTransform(stamp_ns, T_world_dvs);
+    return was_reset;
+  }
+  // getPoseAt (:709-744): the tf pose; with dvs_frame_id "marker" the rpg rig's ground truth is the marker's pose and the
+  // camera's is T_world_marker * T_marker_cam (the constant of :731-735).
+  bool getPoseAt(int64_t t_ns, esvo::Pose& T) const {
+    esvo::Pose Tm;
+    if (!tf_.lookup(t_ns, Tm)) return false;
+    if (!marker_frame_) { T = Tm; return true; }
+    static constexpr double Mc[16] = {5.363262328777285e-01, -1.748374625145743e-02, -8.438296573030597e-01, -7.009849865398374e-02,
+                                      8.433577587813513e-01, -2.821937531845164e-02, 5.366109927684415e-01, 1.881333563905305e-02,
+                                      -3.319431623758162e-02, -9.994488408486204e-01, -3.897382049768972e-04, -6.966829200678797e-02,
+                                      0, 0, 0, 1};
+    for (int r = 0; r < 4; ++r)
+      for (int c = 0; c < 4; ++c) T[4 * r + c] = Tm[4 * r] * Mc[c] + Tm[4 * r + 1] * Mc[4 + c] + Tm[4 * r + 2] * Mc[8 + c] + Tm[4 * r + 3] * Mc[12 + c];
+    return true;
+  }
+  // reset (:840-880): events, history, tf and TS_id_ here; the owner drops the map and the fusion window.  Not restated:
+  // :862-864 re-arm the block matcher in modes 1 and 2 with the unclamped BM_min_disparity / BM_max_disparity, so after a
+  // reset the reference's mode 1 searches [BM_min, BM_max] instead of the range the constructor clamps to the inverse-depth
+  // limits (rpg: 1..40 instead of 4..40).  The disparity range is fixed when the context is made; here it stays clamped.
+  void reset() {
+    events_left_.clear(); events_right_.clear(); TS_history_.clear(); tf_.clear(); TS_id_ = 0;
+    ++n_resets_;
+  }
+
+  // dataTransferring (:552-668).  TS_obs_: the newest entry but one, walking back to the oldest, that tf has a pose for.
+  // Then the mode's window: EM frontend::selectEMEvents over [oldest TS, newest TS) on both queues (false: no events);
+  // SGM frontend::selectSGMEvents (2 * BM_half_slice_thickness, `<=`); BM frontend::selectCloseEvents with the cap of
+  // MAX_NUM_Event_INVOLVED (10 * BM_half_slice_thickness) into vALLEventsPtr_left_ and vCloseEventsPtr_left_, and the
+  // virtual-view poses at frontend::samplePoseStamps, a stamp tf has no pose for being skipped.
+  bool dataTransferring() {
+    clearSelection();
+    if (TS_history_.size() <= 10) return false;
+    auto it_end = TS_history_.rbegin();
+    ++it_end;                                             // in case the tf is behind the most current TS
+    const int64_t t_oldest = TS_history_.begin()->first;
+    while (!has_obs_) {
+      esvo::Pose tr;
+      if (getPoseAt(it_end->first, tr)) {
+        TS_obs_.first = it_end->first;
+        TS_obs_.second.left = it_end->second.left.data(); TS_obs_.second.right = it_end->second.right.data();
+        TS_obs_.second.id_ = it_end->second.id; TS_obs_.second.setTransformation(tr);
+        has_obs_ = true;
+      }
+      if (it_end->first == t_oldest) break;
+      ++it_end;
+    }
+    if (!has_obs_) return false;
+    if (msm_ == 0 || msm_ == 2) {
+      t_lowBound_ = TS_history_.begin()->first; t_upBound_ = TS_history_.rbegin()->first;
+      std::vector<esvo::Event*> l, r;
+      if (!frontend::selectEMEvents(events_left_, t_lowBound_, t_upBound_, EM_numEventMatching_, l) ||
+          !frontend::selectEMEvents(events_right_, t_lowBound_, t_upBound_, EM_numEventMatching_, r))
+        return false;
+      vEventsPtr_left_.swap(l); vEventsPtr_right_.swap(r);
+    }
+    if (msm_ == 4)
+      frontend::selectSGMEvents(events_left_, TS_obs_.first, BM_half_slice_thickness_, PROCESS_EVENT_NUM_, vEventsPtr_left_SGM_);
+    if (msm_ == 1 || msm_ == 3) {
+      frontend::selectCloseEvents(events_left_, TS_obs_.first, BM_half_slice_thickness_, MAX_NUM_Event_INVOLVED, vCloseEventsPtr_left_);
+      vALLEventsPtr_left_ = vCloseEventsPtr_left_;        // both are filled by the same walk (:642-647)
+      for (int64_t t : frontend::samplePoseStamps(TS_obs_.first, BM_half_slice_thickness_)) {
+        esvo::Pose tr;
+        if (getPoseAt(t, tr)) st_map_.push_back({t, tr});
+      }
+    }
+    return true;
+  }
+  // The BM branch of MappingAtTime before the matcher (:385-405): the denoising mask of all window events keeps at most
+  // PROCESS_EVENT_NUM of the close events, or, without denoising, the first PROCESS_EVENT_NUM of them.
+  void denoise() {
+    vDenoisedEventsPtr_left_.clear();
+    if (bDenoising_) {
+      std::vector<uint8_t> mask;
+      frontend::createDenoisingMask(vALLEventsPtr_left_, mask, H_, W_);
+      frontend::extractDenoisedEvents(vCloseEventsPtr_left_, vDenoisedEventsPtr_left_, mask, W_, PROCESS_EVENT_NUM_);
+    } else {
+      vDenoisedEventsPtr_left_.assign(vCloseEventsPtr_left_.begin(),
+                                      vCloseEventsPtr_left_.begin() + (long)std::min(vCloseEventsPtr_left_.size(), PROCESS_EVENT_NUM_));
+    }
+  }
+  // The host part of one MappingLoop pass (:196-225): the TS_history_.size() >= 10 gate, dataTransferring, the skip when no
+  // observation was loaded (TS_obs_ empty), and in BM modes the denoising.  true: MappingAtTime is due on TS_obs_ -- also
+  // when dataTransferring returned false after loading the observation (the loop tests TS_obs_, not the return value).
+  struct Pass { bool gated = false, transferred = false, has_obs = false; };
+  bool prepare(Pass& p) {
+    p = Pass();
+    if (TS_history_.size() < 10) { clearSelection(); return false; }
+    p.gated = true;
+    p.transferred = dataTransferring();
+    p.has_obs = has_obs_;
+    if (!has_obs_) return false;
+    if (msm_ == 1 || msm_ == 3) denoise();
+    return true;
+  }
+
+  std::deque<esvo::Event> events_left_, events_right_;   // EventQueue
+  struct TsPair { std::vector<uint8_t> left, right; size_t id; };
+  std::map<int64_t, TsPair> TS_history_;
+  size_t TS_id_ = 0, n_resets_ = 0;
+  esvo::PoseBuffer tf_;
+  int64_t tf_latest_common_time_ = 0;
+  // what dataTransferring / denoise leave
+  esvo::StampedTimeSurfaceObs TS_obs_;
+  bool has_obs_ = false;
+  std::vector<esvo::Event*> vEventsPtr_left_, vEventsPtr_right_, vEventsPtr_left_SGM_, vALLEventsPtr_left_, vCloseEventsPtr_left_,
+      vDenoisedEventsPtr_left_;
+  int64_t t_lowBound_ = 0, t_upBound_ = 0;
+  esvo::StampTransformationMap st_map_;
+  size_t W_, H_;
+  int msm_;
+ private:
+  // The observation and every selection are cleared at the start of a pass: a pass without an observation leaves nothing
+  // behind (the reference keeps the previous pass's pointers there, which nothing reads, and a reset leaves them dangling).
+  void clearSelection() {
+    TS_obs_ = esvo::StampedTimeSurfaceObs(); has_obs_ = false;
+    for (auto* v : {&vEventsPtr_left_, &vEventsPtr_right_, &vEventsPtr_left_SGM_, &vALLEventsPtr_left_, &vCloseEventsPtr_left_,
+                    &vDenoisedEventsPtr_left_})
+      v->clear();
+    st_map_.clear();
+  }
+  static bool inconsistent(int64_t t_new, int64_t t_old) {   // max_time_diff_before_reset_s = 0.5
+    const double dt = frontend::toSec(t_new) - frontend::toSec(t_old);
+    return dt < 0 || std::fabs(dt) >= 0.5;
+  }
+};
+
 // esvo_core::esvo_MVStereo::MappingAtTime (esvo_MVStereo.cpp:239-520): the known-pose multi-view-stereo node the reference
 // uses to compare five depth estimators on the same fusion back-end.  The node's dataTransferring (:544-668) fills the
 // public input members below (front-end helpers: frontend::selectCloseEvents / samplePoseStamps / eventSlicingForEM);
@@ -702,7 +983,7 @@ class esvo_MVStereo {
   enum eMVStereoMode { PURE_EVENT_MATCHING, PURE_BLOCK_MATCHING, EM_PLUS_ESTIMATION, BM_PLUS_ESTIMATION, PURE_SEMI_GLOBAL_MATCHING };   // esvo_MVStereo.h:38-45
   using PoseProvider = std::function<bool(int64_t, esvo::Pose&)>;
   esvo_MVStereo(esvo::CameraSystem::Ptr cs, eMVStereoMode msm, size_t NUM_THREAD_MAPPING = 4)
-      : msm_(msm), em_(cs, NUM_THREAD_MAPPING), ebm_(cs), dpSolver_(cs), dFusor_(cs), dRegularizor_(cs), cs_(cs) {
+      : node_(cs->width_, cs->height_, (int)msm), msm_(msm), em_(cs, NUM_THREAD_MAPPING), ebm_(cs), dpSolver_(cs), dFusor_(cs), dRegularizor_(cs), cs_(cs) {
     const esvo_params& p = cs_->params();
     em_.resetParameters(EM_Time_THRESHOLD_, EM_EPIPOLAR_THRESHOLD_, EM_TS_NCC_THRESHOLD_, (size_t)p.patch_size_x, (size_t)p.patch_size_y, 125, 0.1);   // :85-91
     maxNumFusionFrames_ = (size_t)p.max_num_fusion_frames; maxNumFusionPoints_ = (size_t)p.max_num_fusion_points;
@@ -780,11 +1061,81 @@ class esvo_MVStereo {
   }
   void getElements(std::vector<esvo::DepthPoint>& out) { dFusor_.getElements(out); }
   void reset() { dqvDepthPoints_.clear(); }
+
+  // ---- the node around MappingAtTime: callbacks, getPoseAt, dataTransferring, one pass of MappingLoop and the publishers
+  // (esvo_MVStereo.cpp:179-237,552-880,960-1055).  The host logic is node_ (MVStereoFrontEnd); a reset it reports also
+  // empties the map and drops the fusion window, as reset() (:840-880) does with depthFramePtr_ and dqvDepthPoints_.
+  // The owner sets node_'s parameters and points the pose provider at getPoseAt (the EM slices look their poses up there).
+  MVStereoFrontEnd node_;
+  void eventsCallback(const std::vector<esvo::Event>& events, bool left) { if (node_.eventsCallback(events, left)) resetMap(); }
+  void timeSurfaceCallback(int64_t stamp_ns, const uint8_t* ts_left, const uint8_t* ts_right) {
+    if (node_.timeSurfaceCallback(stamp_ns, ts_left, ts_right)) resetMap();
+  }
+  void stampedPoseCallback(int64_t stamp_ns, const esvo::Pose& T_world_dvs) { if (node_.stampedPoseCallback(stamp_ns, T_world_dvs)) resetMap(); }
+  bool getPoseAt(int64_t t_ns, esvo::Pose& T) const { return node_.getPoseAt(t_ns, T); }
+  // dataTransferring (:552-668) into the inputs above; BM modes get the window events undenoised (see MappingLoopOnce)
+  bool dataTransferring() {
+    const bool ok = node_.dataTransferring();
+    takeInputs(node_.vCloseEventsPtr_left_);
+    return ok;
+  }
+  // What one pass of MappingLoop did.  gated: TS_history_.size() >= 10; transferred: dataTransferring's result; ran:
+  // MappingAtTime was called (an observation was loaded -- publishKFPose then published stamp / T_world_kf); ok: it
+  // reached the accumulation / fusion; published: publishPointCloud published `cloud` (world frame, f32 x,y,z).
+  struct LoopResult {
+    bool gated = false, transferred = false, ran = false, ok = false, published = false;
+    int64_t stamp = 0; esvo::Pose T_world_kf{};
+    size_t n_left = 0, n_right = 0, n_sgm = 0, n_window = 0, n_close = 0, n_st = 0, n_matches = 0;
+    std::vector<float> cloud;
+  };
+  // one pass of MappingLoop's body (:196-225) with publishMappingResults / publishPointCloud (:960-1039) run in line
+  bool MappingLoopOnce(LoopResult& res) {
+    res = LoopResult();
+    MVStereoFrontEnd::Pass p;
+    const bool due = node_.prepare(p);
+    res.gated = p.gated; res.transferred = p.transferred;
+    if (!due) return false;
+    takeInputs(node_.vDenoisedEventsPtr_left_);
+    res.stamp = TS_obs_.first; res.T_world_kf = TS_obs_.second.tr_;                        // publishKFPose (:1041-1055)
+    res.n_left = vEventsPtr_left_.size(); res.n_right = vEventsPtr_right_.size(); res.n_sgm = vEventsPtr_left_SGM_.size();
+    res.n_window = node_.vALLEventsPtr_left_.size(); res.n_close = vCloseEventsPtr_left_.size(); res.n_st = st_map_.size();
+    res.ran = true;
+    res.ok = MappingAtTime();
+    res.n_matches = vEMP_.size();
+    if (res.ok) publishMappingResults(res);
+    return res.ok;
+  }
+  // The map of the current DepthFrame: empty when none has been filled since it was made (a MappingAtTime that returned
+  // before the accumulation, or a reset).
+  void getMap(std::vector<esvo::DepthPoint>& out) {
+    if (!depthFramePtr_ || depthFramePtr_->fresh_) { out.clear(); return; }
+    getElements(out);
+  }
   eMVStereoMode msm_;
   double EM_Slice_Thickness_ = 1e-3, EM_Time_THRESHOLD_ = 5e-5, EM_EPIPOLAR_THRESHOLD_ = 0.5, EM_TS_NCC_THRESHOLD_ = 0.1;   // :81-84
   size_t num_disparities_ = 16 * 3, block_size_ = 11, P1_ = 8 * 11 * 11, P2_ = 32 * 11 * 11;                                // :100-107
   size_t maxNumFusionFrames_ = 20, maxNumFusionPoints_ = 2000;
  private:
+  void takeInputs(const std::vector<esvo::Event*>& bm_events) {
+    TS_obs_ = node_.TS_obs_;
+    vEventsPtr_left_ = node_.vEventsPtr_left_; vEventsPtr_right_ = node_.vEventsPtr_right_;
+    t_lowBound_ = node_.t_lowBound_; t_upBound_ = node_.t_upBound_;
+    vEventsPtr_left_SGM_ = node_.vEventsPtr_left_SGM_;
+    vCloseEventsPtr_left_ = bm_events;
+    st_map_ = node_.st_map_;
+  }
+  void resetMap() {
+    dqvDepthPoints_.clear();
+    esvo_mapping_reset(cs_->ctx());
+    if (depthFramePtr_) depthFramePtr_->fresh_ = true;   // depthFramePtr_->clear()
+  }
+  // publishMappingResults -> publishPointCloud (:960-1039): the DepthMap at the frame's pose, nothing when it is empty
+  void publishMappingResults(LoopResult& res) {
+    std::vector<esvo::DepthPoint> elems;
+    getMap(elems);
+    frontend::packPointCloud(elems, depthFramePtr_->T_world_frame_, res.cloud);
+    res.published = !res.cloud.empty();
+  }
   // accumulation of modes 0, 1, 4 (:280-286,355-361,423-427): window of maxNumFusionFrames_ vectors, newest first, nearest wins
   bool accumulateNaive(std::vector<esvo::DepthPoint>& vdp) {
     dqvDepthPoints_.push_back(vdp);

@@ -18,75 +18,7 @@
 
 #include "esvo_core.hpp"
 
-namespace esvo {
-
-// The tf::Transformer(true, ros::Duration(100.0)) both nodes keep (esvo_Mapping.cpp:140, esvo_Tracking.cpp:58), filled by
-// stampedPoseCallback and read by getPoseAt.  Restates the tf2 TimeCache behaviour the nodes rely on (DESIGN.md section 2):
-//  * the pose travels as quaternion + position (PoseStamped) and comes back as a 4x4: q = Eigen::Quaterniond(R) on the way
-//    in, R = q.toRotationMatrix() on the way out -- an exact stamp returns the stored pose after that round trip;
-//  * between two stamps: translation (1 - r) p0 + r p1, rotation tf2 slerp (shortest path), r = (t - t0) / (t1 - t0) in
-//    seconds of ros::Duration;
-//  * no extrapolation: before the oldest or after the newest stamp there is no pose; one entry answers only at its stamp;
-//    stamp 0 means "the latest";
-//  * entries older than the newest minus the cache time (100 s) are dropped; a second pose for a stored stamp is refused.
-class PoseBuffer {
- public:
-  explicit PoseBuffer(int64_t cache_ns = 100000000000LL) : cache_ns_(cache_ns) {}
-  bool setTransform(int64_t stamp_ns, const Pose& T_world_dvs) {
-    if (!s_.empty() && s_.back().t > stamp_ns + cache_ns_) return false;
-    auto it = std::lower_bound(s_.begin(), s_.end(), stamp_ns, [](const Entry& e, int64_t t) { return e.t < t; });
-    if (it != s_.end() && it->t == stamp_ns) return false;
-    Entry e;
-    e.t = stamp_ns;
-    const double R[9] = {T_world_dvs[0], T_world_dvs[1], T_world_dvs[2], T_world_dvs[4], T_world_dvs[5], T_world_dvs[6],
-                         T_world_dvs[8], T_world_dvs[9], T_world_dvs[10]};
-    quaternionFromRotation(R, e.q);
-    e.p[0] = T_world_dvs[3]; e.p[1] = T_world_dvs[7]; e.p[2] = T_world_dvs[11];
-    s_.insert(it, e);
-    while (s_.front().t + cache_ns_ < s_.back().t) s_.erase(s_.begin());
-    return true;
-  }
-  bool canTransform(int64_t t_ns) const { Pose T; return lookup(t_ns, T); }
-  bool lookup(int64_t t_ns, Pose& T) const {
-    if (s_.empty()) return false;
-    if (t_ns == 0) return toPose(s_.back().q, s_.back().p, T);
-    if (t_ns < s_.front().t || t_ns > s_.back().t) return false;
-    auto it = std::upper_bound(s_.begin(), s_.end(), t_ns, [](int64_t t, const Entry& e) { return t < e.t; });
-    const Entry& a = *(it - 1);
-    if (a.t == t_ns) return toPose(a.q, a.p, T);
-    const Entry& b = *it;
-    const double r = esvo_core::frontend::toSec(t_ns - a.t) / esvo_core::frontend::toSec(b.t - a.t);   // ros::Duration::toSec()
-    double q[4], p[3];
-    for (int i = 0; i < 3; ++i) p[i] = (1.0 - r) * a.p[i] + r * b.p[i];
-    slerp(a.q, b.q, r, q);
-    return toPose(q, p, T);
-  }
-  size_t size() const { return s_.size(); }
-  void clear() { s_.clear(); }
-  // tf2::Quaternion::slerp / angleShortestPath (tf2Acos clamps to [-1, 1]); q = x, y, z, w
-  static void slerp(const double a[4], const double b[4], double t, double out[4]) {
-    auto dot = [](const double* u, const double* v) { return u[0] * v[0] + u[1] * v[1] + u[2] * v[2] + u[3] * v[3]; };
-    const double s = std::sqrt(dot(a, a) * dot(b, b)), d_ab = dot(a, b);
-    const double c = std::max(-1.0, std::min(1.0, (d_ab < 0 ? -d_ab : d_ab) / s));
-    const double theta = std::acos(c) * 2.0 / 2.0;
-    if (theta == 0.0) { std::copy(a, a + 4, out); return; }
-    const double d = 1.0 / std::sin(theta), s0 = std::sin((1.0 - t) * theta), s1 = std::sin(t * theta);
-    const double sg = d_ab < 0 ? -1.0 : 1.0;
-    for (int i = 0; i < 4; ++i) out[i] = (a[i] * s0 + sg * b[i] * s1) * d;
-  }
- private:
-  struct Entry { int64_t t; double q[4]; double p[3]; };
-  static bool toPose(const double q[4], const double p[3], Pose& T) {
-    double R[9];
-    rotationFromQuaternion(q, R);
-    T = {R[0], R[1], R[2], p[0], R[3], R[4], R[5], p[1], R[6], R[7], R[8], p[2], 0, 0, 0, 1};
-    return true;
-  }
-  int64_t cache_ns_;
-  std::vector<Entry> s_;   // oldest first
-};
-
-}  // namespace esvo
+// esvo::PoseBuffer, the tf pose buffer both nodes look poses up in, lives in esvo_core.hpp (the MVStereo node owns one too).
 
 namespace esvo_core {
 
