@@ -63,12 +63,18 @@ __device__ __forceinline__ double em_patch_at(const EmPatch& p, int pitch, int y
   return p.q3 * r0 + p.q4 * r1;
 }
 
+// PerspectiveCamera::cam2World in the reference's literal form (4x4 cofactor inverse, fuse.cu).  Here and in
+// seeds_to_points_kernel the point is re-projected right away: with an integral rectified coordinate and T_left_rv = I the
+// re-projection sits exactly on a pixel boundary, so the last bit of p decides the patch's base pixel and the warp's border
+// tests.  The closed form (x - cx - tx/z) z / fx rounds differently in about half of such warps; this path is not hot.
+__device__ void cam2world_general(const DevConsts& dc, double x, double y, double rho, double& p0, double& p1, double& p2);   // fuse.cu
+
 // warping2 (:276-306) + the two patchInterpolation2 + zncc_cost (:253-274) for one candidate depth
 __device__ bool em_candidate_cost(const DevConsts& dc, const EmArgs& a, const double* T /*3x4, shared*/, double xl0, double xl1, double inv_depth,
                                   double& cost) {
   const int wx = a.wx, wy = a.wy;
-  const double z = 1.0 / inv_depth;                    // PerspectiveCamera::cam2World, closed form (see lm.cu)
-  const double p0 = (xl0 - dc.cx - dc.Pl[3] / z) * z / dc.fx, p1 = (xl1 - dc.cy - dc.Pl[7] / z) * z / dc.fy, p2 = z * (1.0 - dc.Pl[11] / z);
+  double p0, p1, p2;
+  cam2world_general(dc, xl0, xl1, inv_depth, p0, p1, p2);
   double pl[3];
 #pragma unroll
   for (int q = 0; q < 3; ++q) pl[q] = T[q * 4 + 0] * p0 + T[q * 4 + 1] * p1 + T[q * 4 + 2] * p2 + T[q * 4 + 3];
@@ -224,10 +230,9 @@ __global__ void __launch_bounds__(kEmOrdBlock) em_order_kernel(DevConsts dc, EmA
   if (v0 + kEmOrdBlock >= n && threadIdx.x == 0) a.counters[1] = (unsigned long long)(s_base + total);
 }
 
-// esvo_MVStereo::vEMP2vDP (esvo_MVStereo.cpp:1072-1097).  cam2World in the reference's literal form (4x4 cofactor inverse,
-// fuse.cu): the SGM mode feeds integer pixel coordinates through here, whose re-projection sits exactly on a pixel boundary,
-// so the last bit of p_cam decides which pixels the point lands on.
-__device__ void cam2world_general(const DevConsts& dc, double x, double y, double rho, double& p0, double& p1, double& p2);   // fuse.cu
+// esvo_MVStereo::vEMP2vDP (esvo_MVStereo.cpp:1072-1097).  cam2World in the literal form (above): the SGM mode feeds integer
+// pixel coordinates through here, whose re-projection sits exactly on a pixel boundary, so the last bit of p_cam decides
+// which pixels the point lands on.
 __global__ void seeds_to_points_kernel(DevConsts dc, const esvo_seed* __restrict__ seeds, int n, long long age, esvo_depth_point* out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;

@@ -339,6 +339,21 @@ def em_zncc_cost(pl, pr):
     return 0.5 * (1.0 - float((ln * rn).sum()))
 
 
+def _patch_fail_reason(loc, wx, wy, W, H):
+    """Which test of patch_interpolation rejects loc: "ul" (ulx / uly < 0), "dr" (drx >= W / dry >= H), or "far_y" /
+    "far_x" (only uly + wy >= H / only ulx + wx >= W: the row / column the bilinear weights reach beyond the window), or
+    "far_xy" (both)."""
+    fx, fy = int(np.floor(loc[0])), int(np.floor(loc[1]))
+    ulx, uly = fx - (wx - 1) // 2, fy - (wy - 1) // 2
+    if ulx < 0 or uly < 0:
+        return "ul"
+    if fx + (wx - 1) // 2 >= W or fy + (wy - 1) // 2 >= H:
+        return "dr"
+    if uly + wy >= H:
+        return "far_xy" if ulx + wx >= W else "far_y"
+    return "far_x"
+
+
 def event_slicing_for_em(t_left, t_low_ns, t_up_ns, slice_thickness):
     """esvo_MVStereo::eventSlicingForEM (esvo_MVStereo.cpp:1008-1040) over the time-ordered left events vEventsPtr_left_:
     numSlice = floor((t_up - t_low) / thickness); a slice runs from its first event to lower_bound(first stamp + thickness)
@@ -363,13 +378,23 @@ def event_slicing_for_em(t_left, t_low_ns, t_up_ns, slice_thickness):
 
 
 def event_match(left, right, slice_counts, slice_poses, lut_l, lut_r, Pl, Pr, baseline, ts_l, ts_r, T_world_left,
-                time_thr, epi_thr, ncc_thr, wx, wy, num_thread):
+                time_thr, epi_thr, ncc_thr, wx, wy, num_thread, info=None):
     """EventMatcher::match_all_HyperThread / match / match_an_event (:60-163,185-251).  left / right: dicts of x, y, t, p
-    (right time-ordered).  Returns a list of dicts in the reference's thread-major order and the number of zncc evaluations."""
+    (right time-ordered).  Returns a list of dicts in the reference's thread-major order and the number of zncc evaluations.
+    info (dict, optional) receives counts of the decisions taken: winners by (lane, pass) of a 32-wide scan from the window's
+    first candidate, exact cost ties with the winner, the no-candidate-scored fallback, epipolar decisions exactly at their
+    bounds, candidates exactly on a window bound, and the patch test that rejected a warp."""
     H, W = ts_l.shape
     tsl = ts_l.astype(np.float64); tsr = ts_r.astype(np.float64)
-    slice_of = np.repeat(np.arange(len(slice_counts)), slice_counts)
+    # EventSlice::numEvents_ is a size_t filled from an int: a non-positive count adds no event to the slice loop
+    slice_of = np.repeat(np.arange(len(slice_counts)), np.maximum(np.asarray(slice_counts, np.int64), 0))
     total = min(slice_of.size, left["x"].size)
+    census = dict(winners=[], ties=0, fallback_accept=0, fallback_reject=0, epi_eq_accept=0, epi_ulp_reject=0, disp_zero_reject=0,
+                  disp_ulp_accept=0, on_low=0, on_up=0, warp_fail=0, patch_fail_ul=0, patch_fail_dr=0, patch_fail_far_y=0,
+                  patch_fail_far_x=0, patch_fail_far_xy=0, total=total, num_thread=num_thread)
+    if info is not None:
+        info.update(census)
+        census = info
     r_secs = np.array([ros_to_sec(t) for t in right["t"]])
     T_left_world = np.linalg.inv(np.asarray(T_world_left, float).reshape(4, 4))
     hx, hy = (wx - 1) // 2, (wy - 1) // 2
@@ -381,13 +406,20 @@ def event_match(left, right, slice_counts, slice_poses, lut_l, lut_r, Pl, Pr, ba
         low = ros_to_sec(ros_from_sec(te - time_thr / 2)); up = ros_to_sec(ros_from_sec(te + time_thr / 2))
         b = int(np.searchsorted(r_secs, low, side="left")); e = int(np.searchsorted(r_secs, up, side="left"))
         cand = [j for j in range(b, e) if low <= r_secs[j] <= up and bool(right["p"][j]) == bool(left["p"][i])]     # temporal + polarity (:66-88)
+        census["on_low"] += sum(r_secs[j] == low for j in cand)
+        census["on_up"] += int(np.sum(r_secs[e:] == up))             # `<= up` would take them; lower_bound(up) never offers them
         if not cand:
             return None
         xl = lut_l[int(left["y"][i]), int(left["x"][i])]
         epi = []
         for j in cand:                                                                                               # epipolar (:93-108)
             xr = lut_r[int(right["y"][j]), int(right["x"][j])]
-            if abs(xl[1] - xr[1]) <= epi_thr and xr[0] < xl[0]:
+            dy = abs(xl[1] - xr[1])
+            census["epi_eq_accept"] += bool(dy == epi_thr and xr[0] < xl[0])
+            census["epi_ulp_reject"] += bool(dy == np.nextafter(epi_thr, np.inf) and xr[0] < xl[0])
+            census["disp_zero_reject"] += bool(dy <= epi_thr and xr[0] == xl[0])
+            census["disp_ulp_accept"] += bool(dy <= epi_thr and xr[0] == np.nextafter(xl[0], -np.inf))
+            if dy <= epi_thr and xr[0] < xl[0]:
                 epi.append((j, xr))
         if not epi:
             return None
@@ -395,6 +427,7 @@ def event_match(left, right, slice_counts, slice_poses, lut_l, lut_r, Pl, Pr, ba
         T_left_rv = T_left_world @ T_world_rv
         f = Pl[0, 0]
         min_cost, best, best_depth = 1.0, 0, 0.0
+        costs = []
         for q, (j, xr) in enumerate(epi):                                                                            # motion check (:110-150)
             depth = baseline * f / (xl[0] - xr[0])
             p_rv = cam2world(Pl, xl, 1.0 / depth)
@@ -402,14 +435,25 @@ def event_match(left, right, slice_counts, slice_poses, lut_l, lut_r, Pl, Pr, ba
             h1 = Pl[:, :3] @ p_left + Pl[:, 3]; h2 = Pr[:, :3] @ p_left + Pr[:, 3]
             x1 = h1[:2] / h1[2]; x2 = h2[:2] / h2[2]
             if any(xs[0] < hx or xs[0] > W - hx or xs[1] < hy or xs[1] > H - hy for xs in (x1, x2)):               # warping2 (:276-306)
+                census["warp_fail"] += 1
                 continue
             pa = patch_interpolation(tsl, x1, wx, wy)
             pb = patch_interpolation(tsr, x2, wx, wy) if pa is not None else None
             if pa is None or pb is None:
+                census["patch_fail_" + _patch_fail_reason(x1 if pa is None else x2, wx, wy, W, H)] += 1
                 continue
             cost = em_zncc_cost(pa, pb); evals += 1
+            costs.append(cost)
             if cost < min_cost:
                 min_cost, best, best_depth = cost, q, depth
+        if min_cost < 1.0:
+            census["ties"] += sum(c == min_cost for c in costs) - 1
+            k = epi[best][0] - b
+            census["winners"].append((k % 32, k // 32 + 1))
+        elif min_cost <= ncc_thr:
+            census["fallback_accept"] += 1
+        else:
+            census["fallback_reject"] += 1
         if min_cost > ncc_thr:
             return None
         with np.errstate(divide="ignore"):

@@ -26,24 +26,29 @@ STREAMS = {"rpg": dict(depth_range=(0.8, 3.0), n_segments=40), "upenn": dict(dep
 QUALITY = {"rpg": {0: 0.048, 1: 0.057, 2: 0.38, 3: 0.05, 4: 0.065}, "upenn": {0: 0.09, 1: 0.073, 2: 0.033, 3: 0.024, 4: 0.066}}
 # Product against oracle over a whole stream.  Modes 0 (EM) and 4 (SGM) are compared end to end: the bar of
 # tests/test_gpu_mvstereo.py at every mapping tick (element order, rows / cols / ages exact, values within 1e-9).  In modes 1-3
-# an end-to-end comparison amplifies legitimate ties.  The matcher's cost agrees with the oracle's to ~1e-16, not to the bit
+# an end-to-end comparison amplifies legitimate ties.  The block matcher's cost agrees with the oracle's to ~1e-16, not to the bit
 # (the ZNCC sums run in another order), and the naive propagation keeps a point only for a strictly smaller residual.  So two
 # seeds with equal inverse depth that the product scores with the very same cost, and the oracle 5.5e-17 apart, pick
 # different winners (rpg mode 1, tick 35: 2 of 846 elements), and later frames build
 # on that pixel.  The LM's own 1e-4 tail does the same through the fusion's thresholds.  There each stage is held to its bar
 # on identical inputs: the oracle's matcher (and LM) output is checked against the product's at the bar of
-# tests/test_gpu_mvstereo.py (seeds exact but the cost, within 1e-9; LM: the same points per pass, inverse depth within 1e-4
+# tests/test_gpu_mvstereo.py (event-matcher seeds exact, cost included, measured over both streams on an H100 80GB HBM3 at
+# 700 W; block-matching seeds exact but the cost, within 1e-9; LM: the same points per pass, inverse depth within 1e-4
 # for >= 99.5 % over the stream), and the product's output is handed on, so every map downstream must meet the end-to-end bar.
 SUBSTITUTED = {1: ("bm_match",), 2: ("em_match", "depth_solve"), 3: ("bm_match", "depth_solve")}
 
 
-def _check_seeds(sg, so):
-    """tests/test_gpu_mvstereo.py's matcher bar."""
+def _check_seeds(sg, so, exact_cost):
+    """tests/test_gpu_mvstereo.py's matcher bar: the event matcher's seeds are exact, cost included; the block matcher's
+    cost is within 1e-9 (it is evaluated from integer moments, DESIGN deviation 1)."""
     assert sg.size == so.size
     assert np.array_equal(so["t_ns"], sg["t_ns"]), "event order differs"
     for f in ("x_left_raw", "x_left", "x_right", "T_world_virtual", "disp", "inv_depth"):
         assert np.array_equal(so[f], sg[f]), f
-    assert np.allclose(sg["cost"], so["cost"], rtol=0, atol=1e-9)
+    if exact_cost:
+        assert np.array_equal(sg["cost"], so["cost"]), "cost"
+    else:
+        assert np.allclose(sg["cost"], so["cost"], rtol=0, atol=1e-9)
 
 
 def _check_lm(pg, po, rels):
@@ -75,7 +80,7 @@ def _substitute(be, names, product_out, rels):
             if _n == "depth_solve":
                 _check_lm(theirs[0], mine[0], rels)
             else:
-                _check_seeds(theirs[0], mine[0])
+                _check_seeds(theirs[0], mine[0], exact_cost=_n == "em_match")
                 assert theirs[1] == mine[1], "matcher evaluations"
             return theirs
         setattr(be, name, w)
