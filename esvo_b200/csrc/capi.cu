@@ -194,6 +194,22 @@ static int stage_mapping(Ctx* c, const uint16_t* ex, const uint16_t* ey, const i
   return stage_inputs_packed(c, ex, ey, et, n, pt, poses, np);
 }
 
+// The part of esvo_set_ts_pair behind the image copies: the observation pose, and the raw pair as the solver's view of it until
+// createMatchProblem smooths it.
+static int obs_set_pose(Ctx* c, const double T[16]) {
+  const size_t nimg = (size_t)c->dc.pitch * c->dc.H;
+  std::memcpy(c->T_world_left, T, sizeof(c->T_world_left));
+  rigid_inverse(T, c->T_left_world_inv);
+  if (!c->prm.smooth_time_surface) { c->obs_ls = c->obs_l; c->obs_rs = c->obs_r; }
+  else {
+    ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_ls, c->obs_l, nimg, cudaMemcpyDeviceToDevice, c->stream));
+    ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_rs, c->obs_r, nimg, cudaMemcpyDeviceToDevice, c->stream));
+  }
+  ESVO_CUDA_TRY(c, cudaEventRecord(c->slots[c->cur].ev_obs, c->stream));
+  c->obs_set = true;
+  return ESVO_OK;
+}
+
 static int fetch_counters(Ctx* c) {
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->h_counters, c->d_counters, kCounters * 8, cudaMemcpyDeviceToHost, c->stream));
   ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
@@ -362,6 +378,11 @@ ESVO_API void esvo_destroy(esvo_ctx* c) {
   for (auto& f : c->win) { cudaFree(f.pts); cudaFree(f.cnt); if (f.last_read) cudaEventDestroy(f.last_read); }
   for (auto& f : c->win_pool) { cudaFree(f.pts); cudaFree(f.cnt); if (f.last_read) cudaEventDestroy(f.last_read); }
   for (auto e : c->prof_pool) cudaEventDestroy(e);
+  if (c->hist.buf) cudaFree(c->hist.buf);
+  for (auto e : c->hist.ev) cudaEventDestroy(e);
+  if (c->hist.ev_join) cudaEventDestroy(c->hist.ev_join);
+  for (void* p : {(void*)c->pub.xyz, (void*)c->pub.sorted, (void*)c->pub.d_scal}) if (p) cudaFree(p);
+  if (c->pub.h_scal) cudaFreeHost(c->pub.h_scal);
   if (c->h_stage) cudaFreeHost(c->h_stage);
   for (int k = 0; k < 2; ++k) if (c->s_tsc[k] && c->s_tsc[k] != c->s_main) cudaStreamDestroy(c->s_tsc[k]);
   if (c->ev_ts_join) cudaEventDestroy(c->ev_ts_join);
@@ -498,18 +519,73 @@ ESVO_API int esvo_set_ts_pair(esvo_ctx* c, const uint8_t* l, const uint8_t* r, c
     if (!c->ts[1].built) { c->set_error("ts_right == NULL but no time surface was built for camera 1"); return ESVO_ERR_STATE; }
     if (c->obs_r != c->ts[1].last_img) ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_r, c->ts[1].last_img, nimg, cudaMemcpyDeviceToDevice, c->stream));
   }
-  std::memcpy(c->T_world_left, T, sizeof(c->T_world_left));
-  rigid_inverse(T, c->T_left_world_inv);
-  // Until createMatchProblem smooths it, the observation the solver reads is the raw pair.
-  if (!c->prm.smooth_time_surface) { c->obs_ls = c->obs_l; c->obs_rs = c->obs_r; }
-  else {
-    ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_ls, c->obs_l, nimg, cudaMemcpyDeviceToDevice, c->stream));
-    ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_rs, c->obs_r, nimg, cudaMemcpyDeviceToDevice, c->stream));
-  }
-  ESVO_CUDA_TRY(c, cudaEventRecord(c->slots[c->cur].ev_obs, c->stream));
+  int rc = obs_set_pose(c, T);
+  if (rc) return rc;
   ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));  // the caller's images are host memory
-  c->obs_set = true;
   return ESVO_OK;
+}
+
+// ---- time-surface history (TimeSurfaceHistory, esvo_Mapping.h: std::map<ros::Time, TimeSurfaceObservation>) ----
+ESVO_API int esvo_ts_history_reserve_dev(esvo_ctx* c, size_t capacity) {
+  CHECK_CTX(c);
+  { int rc0 = drain(c); if (rc0) return rc0; }
+  Ctx::TsHistory& h = c->hist;
+  if (h.buf) { cudaFree(h.buf); h.buf = nullptr; }
+  for (auto e : h.ev) cudaEventDestroy(e);
+  h.stamp.clear(); h.used.clear(); h.ev.clear();
+  if (capacity == 0) return ESVO_OK;
+  const size_t nimg = (size_t)c->dc.pitch * c->dc.H;
+  ESVO_CUDA_TRY(c, dmalloc(&h.buf, 2 * capacity * nimg));
+  if (!h.ev_join) ESVO_CUDA_TRY(c, cudaEventCreateWithFlags(&h.ev_join, cudaEventDisableTiming));
+  h.stamp.assign(capacity, 0); h.used.assign(capacity, false); h.ev.assign(capacity, nullptr);
+  for (auto& e : h.ev) ESVO_CUDA_TRY(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  return ESVO_OK;
+}
+ESVO_API int esvo_ts_history_store_dev(esvo_ctx* c, int64_t stamp) {
+  CHECK_CTX(c);
+  Ctx::TsHistory& h = c->hist;
+  if (!h.cap()) { c->set_error("esvo_ts_history_store_dev: no history reserved (esvo_ts_history_reserve_dev)"); return ESVO_ERR_STATE; }
+  if (!c->ts[0].built || !c->ts[1].built) { c->set_error("esvo_ts_history_store_dev needs a built time surface for both cameras"); return ESVO_ERR_STATE; }
+  // operator[] then erase(begin()) while over capacity: a stored stamp is overwritten, a new one takes a free entry or the
+  // one with the smallest stamp -- unless it is itself the smallest, which the map would insert and drop again at once
+  size_t i = h.cap(), oldest = h.cap();
+  for (size_t k = 0; k < h.cap() && i == h.cap(); ++k) if (h.used[k] && h.stamp[k] == stamp) i = k;
+  for (size_t k = 0; k < h.cap() && i == h.cap(); ++k) if (!h.used[k]) i = k;
+  if (i == h.cap()) {
+    for (size_t k = 0; k < h.cap(); ++k) if (oldest == h.cap() || h.stamp[k] < h.stamp[oldest]) oldest = k;
+    if (stamp < h.stamp[oldest]) return ESVO_OK;
+    i = oldest;
+  }
+  const size_t nimg = (size_t)c->dc.pitch * c->dc.H;
+  // Both copies go on camera 0's time-surface stream behind both builds; camera 1's stream waits for them before it may
+  // overwrite its image.  No host sync.
+  cudaStream_t s0 = c->s_tsc[0], s1 = c->s_tsc[1];
+  if (s1 != s0) { ESVO_CUDA_TRY(c, cudaEventRecord(h.ev_join, s1)); ESVO_CUDA_TRY(c, cudaStreamWaitEvent(s0, h.ev_join, 0)); }
+  ESVO_CUDA_TRY(c, cudaStreamWaitEvent(s0, h.ev[i], 0));                  // a hand-over may still be reading the entry
+  ESVO_CUDA_TRY(c, cudaMemcpyAsync(h.buf + 2 * i * nimg, c->ts[0].last_img, nimg, cudaMemcpyDeviceToDevice, s0));
+  ESVO_CUDA_TRY(c, cudaMemcpyAsync(h.buf + (2 * i + 1) * nimg, c->ts[1].last_img, nimg, cudaMemcpyDeviceToDevice, s0));
+  ESVO_CUDA_TRY(c, cudaEventRecord(h.ev[i], s0));
+  if (s1 != s0) ESVO_CUDA_TRY(c, cudaStreamWaitEvent(s1, h.ev[i], 0));
+  h.stamp[i] = stamp; h.used[i] = true;
+  return ESVO_OK;
+}
+ESVO_API int esvo_set_ts_pair_stored_dev(esvo_ctx* c, int64_t stamp, const double T[16]) {
+  CHECK_CTX(c);
+  if (!T) return ESVO_ERR_INVALID_ARG;
+  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  Ctx::TsHistory& h = c->hist;
+  size_t i = h.cap();
+  for (size_t k = 0; k < h.cap(); ++k) if (h.used[k] && h.stamp[k] == stamp) { i = k; break; }
+  if (i == h.cap()) {
+    c->set_error("esvo_set_ts_pair_stored_dev: no time-surface pair is stored under stamp " + std::to_string((long long)stamp));
+    return ESVO_ERR_STATE;
+  }
+  const size_t nimg = (size_t)c->dc.pitch * c->dc.H;
+  ESVO_CUDA_TRY(c, cudaStreamWaitEvent(c->stream, h.ev[i], 0));
+  ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_l, h.buf + 2 * i * nimg, nimg, cudaMemcpyDeviceToDevice, c->stream));
+  ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_r, h.buf + (2 * i + 1) * nimg, nimg, cudaMemcpyDeviceToDevice, c->stream));
+  ESVO_CUDA_TRY(c, cudaEventRecord(h.ev[i], c->stream));
+  return obs_set_pose(c, T);
 }
 
 ESVO_API int esvo_set_ts_pair_dev(esvo_ctx* c, const double T[16]) {

@@ -254,6 +254,28 @@ ESVO_API int esvo_map_download(esvo_ctx* c, esvo_depth_point* out, size_t* n) {
   if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
   return map_download(c, out, n);
 }
+ESVO_API int esvo_map_publish_dev(esvo_ctx* c, const double T[16], int64_t stamp, size_t* n_points) {
+  CHECK_CTX(c);
+  if (!T || !n_points) return ESVO_ERR_INVALID_ARG;
+  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  c->pub.valid = false;
+  int rc = map_publish(c, T, n_points);
+  if (rc) return rc;
+  c->pub.n = *n_points; c->pub.stamp = stamp; c->pub.valid = true;
+  return ESVO_OK;
+}
+ESVO_API int esvo_map_published_cloud_dev(esvo_ctx* c, float* xyz_dev, size_t* n, int64_t* stamp) {
+  CHECK_CTX(c);
+  if (!n) return ESVO_ERR_INVALID_ARG;
+  if (!c->pub.valid) { c->set_error("esvo_map_published_cloud_dev: no cloud was published on this context"); return ESVO_ERR_STATE; }
+  if (c->pub.n > *n) { *n = c->pub.n; return ESVO_ERR_CAPACITY; }
+  if (c->pub.n && !xyz_dev) return ESVO_ERR_INVALID_ARG;
+  if (c->pub.n) ESVO_CUDA_TRY(c, cudaMemcpyAsync(xyz_dev, c->pub.xyz, c->pub.n * 3 * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+  *n = c->pub.n;
+  if (stamp) *stamp = c->pub.stamp;
+  return ESVO_OK;
+}
 ESVO_API int esvo_sgbm_compute(esvo_ctx* c, const uint8_t* left, const uint8_t* right, int num_disparities, int block_size, int P1, int P2,
                                int disp12_max_diff, int pre_filter_cap, int uniqueness_ratio, int16_t* disp16_out) {
   CHECK_CTX(c);

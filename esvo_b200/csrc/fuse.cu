@@ -51,6 +51,7 @@ struct MapState {
   int folds = 0;                 // folds since the last reset
   size_t fold_words = 0;         // bitmap words covering the ids of the first fold after the reset
   bool list_valid = false;       // every existing pixel is in `active` (true from a reset until a kernel that ignores the list runs)
+  bool cleaned = false;          // esvo_map_clean removed elements since the reset: their creator bits are stale
   unsigned long long seq_base = 0;
   double T_world_frame[16];
   double T_frame_world[16];
@@ -895,7 +896,7 @@ int fuse_reset_map(Ctx* c, const double T[16]) {
   for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) I[i * 4 + j] = T[j * 4 + i];
   for (int i = 0; i < 3; ++i) { double s = 0; for (int k = 0; k < 3; ++k) s += I[i * 4 + k] * T[k * 4 + 3]; I[i * 4 + 3] = -s; }
   ms->seq_base = 0; ms->staged = 0;
-  ms->list_valid = true; ms->folds = 0;
+  ms->list_valid = true; ms->folds = 0; ms->cleaned = false;
   return ESVO_OK;
 }
 
@@ -1000,6 +1001,7 @@ int map_clean(Ctx* c, double var_thr, double age_thr, double rmax, double rmin) 
   const int npix = c->dc.W * c->dc.H, B = 256;
   map_clean_kernel<<<div_up(npix, B), B, 0, c->stream>>>(npix, c->map->m, var_thr, age_thr, rmax, rmin);
   c->launches += 1;
+  c->map->cleaned = true;
   return ESVO_OK;
 }
 
@@ -1034,7 +1036,7 @@ int map_gather_async(Ctx* c, esvo_depth_point* d_out, unsigned long long* d_keys
   MapState* ms = c->map;
   const int npix = c->dc.W * c->dc.H, B = 128;
   Pose16 Twf; std::memcpy(Twf.m, ms->T_world_frame, 128);
-  if (h_sorted && list_ok(ms) && ms->fold_words) {
+  if (h_sorted && list_ok(ms) && ms->fold_words && !ms->cleaned) {
     // sort-free: rank from the creator bitmap; the kernels write elements, scalars and counters straight into pinned memory
     map_cbits_prefix_kernel<<<1, 1024, 0, c->stream>>>(ms->cbits, ms->cprefix, (int)ms->fold_words, ms->d_scal, h_scal8, c->d_counters, h_counters);
     map_gather_list_kernel<<<div_up(npix, B), B, 0, c->stream>>>(ms->m, Twf, ms->active, ms->d_scal, ms->cbits, ms->cprefix, h_sorted);
@@ -1053,6 +1055,46 @@ int map_gather_async(Ctx* c, esvo_depth_point* d_out, unsigned long long* d_keys
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(h_scal8 + 4, ms->d_scal, 32, cudaMemcpyDeviceToHost, c->stream));
   if (h_counters) ESVO_CUDA_TRY(c, cudaMemcpyAsync(h_counters, c->d_counters, kCounters * 8, cudaMemcpyDeviceToHost, c->stream));
   ESVO_CUDA_TRY(c, cudaGetLastError());
+  return ESVO_OK;
+}
+
+// publishPointCloud's packing (esvo_Mapping.cpp:909-953, frontend::packPointCloud): p_world = R p_cam + t of every element,
+// in element-list order, as pcl::PointXYZ.  The host code is built without FMA contraction, so each row is summed as
+// ((T0 p0 + T1 p1) + T2 p2) + T3 with separately rounded products and one conversion to f32 at the end: the explicit
+// _rn intrinsics keep that rounding whatever the compiler flags are.
+__global__ void map_pack_cloud_kernel(const esvo_depth_point* __restrict__ e, int n, Pose16 Tp, float* __restrict__ xyz) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double* T = Tp.m;
+  const double* p = e[i].p_cam;
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    const double s = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4 * r], p[0]), __dmul_rn(T[4 * r + 1], p[1])), __dmul_rn(T[4 * r + 2], p[2])),
+                               T[4 * r + 3]);
+    xyz[3 * i + r] = __double2float_rn(s);
+  }
+}
+// Element list in creation order (map_gather_async: creator-bit ranks after one fold, key ranks otherwise), then the pack.
+// One host sync, for the count.
+int map_publish(Ctx* c, const double T[16], size_t* n) {
+  Ctx::Published& pb = c->pub;
+  const size_t npix = (size_t)c->dc.W * c->dc.H;
+  if (!pb.xyz) {
+    ESVO_CUDA_TRY(c, dm(&pb.xyz, 3 * npix)); ESVO_CUDA_TRY(c, dm(&pb.sorted, npix)); ESVO_CUDA_TRY(c, dm(&pb.d_scal, 4));
+    ESVO_CUDA_TRY(c, cudaMallocHost((void**)&pb.h_scal, 8 * 8));
+  }
+  MapState* ms = c->map;
+  int rc = map_gather_async(c, ms->d_dl, ms->d_dl_keys, pb.d_scal, pb.h_scal, pb.sorted, nullptr);
+  if (rc) return rc;
+  ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+  const int cnt = (int)pb.h_scal[1];
+  Pose16 Tp; std::memcpy(Tp.m, T, 128);
+  if (cnt) {
+    map_pack_cloud_kernel<<<div_up(cnt, 128), 128, 0, c->stream>>>(pb.sorted, cnt, Tp, pb.xyz);
+    c->launches += 1;
+    ESVO_CUDA_TRY(c, cudaGetLastError());
+  }
+  *n = (size_t)cnt;
   return ESVO_OK;
 }
 

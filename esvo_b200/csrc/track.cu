@@ -33,11 +33,18 @@ struct TrkDev {
   double* items = nullptr;      // ResItems: numPoints*3 in the ref frame
   double* state = nullptr;      // [0..8] R_, [9..11] t_, [12..27] T_world_ref, [28..43] T_world_left out, [44..46] stats
   size_t cap = 0;
+  // device form (esvo_track_adopt_map_dev / esvo_track_reset_dev): snapshot of a published cloud and the uploaded sample indices
+  float* ref = nullptr; size_t ref_cap = 0;
+  int32_t* idx = nullptr; size_t idx_cap = 0;
 };
 struct TrackState {
   TrkDev d;
   size_t numPoints = 0, numBatches = 1;
   bool ready = false;
+  // The adopted cloud stays where it is; ref->vPointXYZ_'s in-place shuffle becomes this index permutation of it, carried
+  // from reset to reset like the reference's shuffled vector.
+  std::vector<int32_t> perm;
+  bool adopted = false;
   // glibc TYPE_3 rand() state (the reference calls the process-global rand(), RegProblemLM.cpp:49)
   uint32_t hist[31]; int pos = 0;
   void srand_(unsigned s) {
@@ -102,10 +109,13 @@ __global__ void trk_sobel_kernel(const uint8_t* __restrict__ neg, int16_t* __res
   dv[(size_t)y * W + x] = (int16_t)((S(xm, yp) - S(xm, ym)) + 2 * (S(x, yp) - S(x, ym)) + (S(xp, yp) - S(xp, ym)));
 }
 // RegProblemLM::setProblem point transform (:53-54): p_cam = R_world_ref^T (p - t_world_ref)
-__global__ void trk_items_kernel(const float* __restrict__ xyz, int n, const double* __restrict__ Twr, double* __restrict__ items) {
+// idx (device form): point i is xyz[idx[i]], the adopted cloud read through the sampling permutation
+__global__ void trk_items_kernel(const float* __restrict__ xyz, const int32_t* __restrict__ idx, int n, const double* __restrict__ Twr,
+                                 double* __restrict__ items) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const double d0 = (double)xyz[3 * i] - Twr[3], d1 = (double)xyz[3 * i + 1] - Twr[7], d2 = (double)xyz[3 * i + 2] - Twr[11];
+  const size_t k = idx ? (size_t)idx[i] : (size_t)i;
+  const double d0 = (double)xyz[3 * k] - Twr[3], d1 = (double)xyz[3 * k + 1] - Twr[7], d2 = (double)xyz[3 * k + 2] - Twr[11];
 #pragma unroll
   for (int r = 0; r < 3; ++r) items[3 * i + r] = Twr[0 * 4 + r] * d0 + Twr[1 * 4 + r] * d1 + Twr[2 * 4 + r] * d2;
 }
@@ -711,7 +721,7 @@ int track_alloc(Ctx* c) {
 void track_free(Ctx* c) {
   TrackState* t = c->trk;
   if (!t) return;
-  void* ps[] = {t->d.ts, t->d.neg, t->d.du, t->d.dv, t->d.xyz, t->d.items, t->d.state};
+  void* ps[] = {t->d.ts, t->d.neg, t->d.du, t->d.dv, t->d.xyz, t->d.items, t->d.state, t->d.ref, t->d.idx};
   for (void* p : ps) if (p) cudaFree(p);
   delete t;
   c->trk = nullptr;
@@ -733,19 +743,11 @@ static bool inverse4_host(const double* A, double* inv) {
   return true;
 }
 
-}  // namespace esvo
-
-using namespace esvo;
 #define CHECK_CTX(c) do { if (!(c)) return ESVO_ERR_INVALID_ARG; cudaSetDevice((c)->device); } while (0)
 
-extern "C" {
-
-ESVO_API int esvo_track_srand(esvo_ctx* c, unsigned seed) { CHECK_CTX(c); c->trk->srand_(seed); return ESVO_OK; }
-
-ESVO_API int esvo_track_reset(esvo_ctx* c, float* ref_xyz, size_t n, const double Twr[16], const double Twc[16],
-                              const uint8_t* ts_left) {
-  CHECK_CTX(c);
-  if (!ref_xyz || !Twr || !Twc) return ESVO_ERR_INVALID_ARG;
+// resetRegProblem / setProblem for both forms: ref_xyz != NULL is the caller's host cloud of n points, shuffled in place;
+// ref_xyz == NULL is the adopted device cloud, shuffled through TrackState::perm.  Same rand() draws in the same order.
+static int track_reset(esvo_ctx* c, float* ref_xyz, size_t n, const double Twr[16], const double Twc[16], const uint8_t* ts_left) {
   if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
   const esvo_params& p = c->prm;
   if (p.trk_patch_size_x != 1 || p.trk_patch_size_y != 1) { c->set_error("tracking patch must be 1x1 (as in every shipped cfg)"); return ESVO_ERR_UNSUPPORTED; }
@@ -769,30 +771,78 @@ ESVO_API int esvo_track_reset(esvo_ctx* c, float* ref_xyz, size_t n, const doubl
   for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) state[i * 3 + j] = Trl[i * 4 + j]; state[9 + i] = Trl[i * 4 + 3]; }
   std::memcpy(state + 12, Twr, 128);
   std::memcpy(state + 28, Twc, 128);
-  // stochastic sampling: partial Fisher-Yates driven by rand() (:45-50), in place on the caller's cloud
+  // stochastic sampling: partial Fisher-Yates driven by rand() (:45-50), in place on the cloud
   const size_t numPoints = std::min(n, (size_t)p.trk_max_registration_points);
   for (size_t i = 0; i < numPoints; ++i) {
     const size_t j = i + (size_t)t->rand_() % (n - i);
-    for (int k = 0; k < 3; ++k) std::swap(ref_xyz[3 * i + k], ref_xyz[3 * j + k]);
+    if (ref_xyz) for (int k = 0; k < 3; ++k) std::swap(ref_xyz[3 * i + k], ref_xyz[3 * j + k]);
+    else std::swap(t->perm[i], t->perm[j]);
   }
   if (numPoints > d.cap) {
     cudaFree(d.xyz); cudaFree(d.items);
     d.cap = numPoints;
     ESVO_CUDA_TRY(c, dm(&d.xyz, d.cap * 3)); ESVO_CUDA_TRY(c, dm(&d.items, d.cap * 3));
   }
-  ESVO_CUDA_TRY(c, cudaMemcpyAsync(d.xyz, ref_xyz, numPoints * 3 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  if (ref_xyz) ESVO_CUDA_TRY(c, cudaMemcpyAsync(d.xyz, ref_xyz, numPoints * 3 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  else {   // only the sampled indices travel; the cloud itself is never moved
+    if (numPoints > d.idx_cap) { cudaFree(d.idx); d.idx_cap = numPoints; ESVO_CUDA_TRY(c, dm(&d.idx, d.idx_cap)); }
+    ESVO_CUDA_TRY(c, cudaMemcpyAsync(d.idx, t->perm.data(), numPoints * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+  }
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(d.state, state, sizeof(state), cudaMemcpyHostToDevice, c->stream));
-  trk_items_kernel<<<div_up((int)numPoints, 256), 256, 0, c->stream>>>(d.xyz, (int)numPoints, d.state + 12, d.items);
+  trk_items_kernel<<<div_up((int)numPoints, 256), 256, 0, c->stream>>>(ref_xyz ? d.xyz : d.ref, ref_xyz ? nullptr : d.idx, (int)numPoints,
+                                                                       d.state + 12, d.items);
   dim3 b(32, 8), g(div_up(dc.W, 32), div_up(dc.H, 8));
   trk_negative_kernel<<<g, b, 0, c->stream>>>(d.ts, d.neg, dc.W, dc.H, dc.pitch, p.trk_kernel_size);
   trk_sobel_kernel<<<g, b, 0, c->stream>>>(d.neg, d.du, d.dv, dc.W, dc.H, dc.pitch);
   c->launches += 3;
   ESVO_CUDA_TRY(c, cudaGetLastError());
-  ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));   // state[] lives on this stack frame
+  ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));   // state[] and perm live on the host
   t->numPoints = numPoints;
   t->numBatches = std::max(numPoints / (size_t)p.trk_batch_size, (size_t)1);
   t->ready = true;
   return ESVO_OK;
+}
+
+}  // namespace esvo
+
+using namespace esvo;
+
+extern "C" {
+
+ESVO_API int esvo_track_srand(esvo_ctx* c, unsigned seed) { CHECK_CTX(c); c->trk->srand_(seed); return ESVO_OK; }
+
+ESVO_API int esvo_track_reset(esvo_ctx* c, float* ref_xyz, size_t n, const double Twr[16], const double Twc[16],
+                              const uint8_t* ts_left) {
+  CHECK_CTX(c);
+  if (!ref_xyz || !Twr || !Twc) return ESVO_ERR_INVALID_ARG;
+  return track_reset(c, ref_xyz, n, Twr, Twc, ts_left);
+}
+
+ESVO_API int esvo_track_adopt_map_dev(esvo_ctx* c, int64_t stamp, size_t* n_points) {
+  CHECK_CTX(c);
+  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  const Ctx::Published& pb = c->pub;
+  if (!pb.valid || pb.stamp != stamp) {
+    c->set_error("esvo_track_adopt_map_dev: the newest cloud published on this context is not the one of stamp " + std::to_string((long long)stamp));
+    return ESVO_ERR_STATE;
+  }
+  TrackState* t = c->trk;
+  TrkDev& d = t->d;
+  if (pb.n > d.ref_cap) { cudaFree(d.ref); d.ref_cap = pb.n; ESVO_CUDA_TRY(c, dm(&d.ref, 3 * d.ref_cap)); }
+  // a snapshot: the mapper may publish again before the next tracking pass
+  if (pb.n) ESVO_CUDA_TRY(c, cudaMemcpyAsync(d.ref, pb.xyz, pb.n * 3 * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  t->perm.resize(pb.n);
+  for (size_t i = 0; i < pb.n; ++i) t->perm[i] = (int32_t)i;
+  t->adopted = true;
+  if (n_points) *n_points = pb.n;
+  return ESVO_OK;
+}
+
+ESVO_API int esvo_track_reset_dev(esvo_ctx* c, const double Twr[16], const double Twc[16], const uint8_t* ts_left) {
+  CHECK_CTX(c);
+  if (!Twr || !Twc) return ESVO_ERR_INVALID_ARG;
+  if (!c->trk->adopted) { c->set_error("esvo_track_reset_dev: no map adopted (esvo_track_adopt_map_dev)"); return ESVO_ERR_STATE; }
+  return track_reset(c, nullptr, c->trk->perm.size(), Twr, Twc, ts_left);
 }
 
 ESVO_API int esvo_track_solve(esvo_ctx* c, int analytical, double Tout[16], esvo_lm_stats* st) {

@@ -1,7 +1,7 @@
 // The closed stereo-odometry loop (include/esvo_b200/esvo_system.hpp) on a recorded pair of event streams: time surfaces,
 // SGM start-up, mapping and tracking on one GPU, on the fixed tick schedule of esvo_core::esvo_System.  Driven by a binary
 // scenario so that a test can run the same stream through the Python restatement (tests/indep_system.py) and compare.
-// usage: system_loop <scenario.bin> <result.bin> <trajectory.txt>
+// usage: system_loop <scenario.bin> <result.bin> <trajectory.txt> [calls.txt]
 // scenario: i32 W, H, rig (0 hkust); i64 t0_ns, dt_ns; i32 n_ticks, mapping_every, profile (1 = per-stage esvo_profile);
 //           i32 n_overrides, then (i32 key, f64 value) each -- keys: 0 trk_batch_size (BATCH_SIZE), 1 PROCESS_EVENT_NUM,
 //           2 Denoising, 3 INIT_SGM_DP_NUM_THRESHOLD;
@@ -12,6 +12,7 @@
 //           per mapping tick: i32 tick, ran (0 nothing, 1 initialisation, 2 mapping), ok, published; u64 SGM points;
 //                     u64 counters[8] (esvo_mapping_at_time order); u64 published cloud points; i64 cloud stamp;
 //           final map: esvo_depth_point[map size]; f64 wall ms; f64 stage ms[8]; u64 stage launches[8]
+// calls:    one line per call SpinOnce / MappingLoopOnce makes: "<name> <total host ms> <calls>"
 #include <chrono>
 #include <cstdio>
 #include <cstring>
@@ -23,7 +24,7 @@ template <class T> static bool rd(std::ifstream& f, T* p, size_t n) { f.read((ch
 template <class T> static void wr(std::ofstream& o, const T* p, size_t n) { o.write((const char*)p, (std::streamsize)(n * sizeof(T))); }
 
 int main(int argc, char** argv) {
-  if (argc < 4) { std::printf("usage: system_loop <scenario.bin> <result.bin> <trajectory.txt>\n"); return 64; }
+  if (argc < 4) { std::printf("usage: system_loop <scenario.bin> <result.bin> <trajectory.txt> [calls.txt]\n"); return 64; }
   std::ifstream f(argv[1], std::ios::binary);
   int32_t W, H, rig, n_ticks, mapping_every, profile, n_ovr;
   int64_t t0, dt;
@@ -113,6 +114,12 @@ int main(int argc, char** argv) {
   }
   wr(o, map.data(), map.size());
   wr(o, &wall_ms, 1); wr(o, prof_ms, 8); wr(o, prof_n, 8);
+  if (argc > 4) {
+    std::FILE* cf = std::fopen(argv[4], "w");
+    if (!cf) { std::printf("cannot write %s\n", argv[4]); return 66; }
+    for (const auto& e : sys.callTimes().ms) std::fprintf(cf, "%s %.6f %zu\n", e.first.c_str(), e.second.first, e.second.second);
+    std::fclose(cf);
+  }
   size_t n_pose = 0;
   for (const auto& tk : sys.ticks_) n_pose += tk.has_pose ? 1 : 0;
   std::printf("system loop: %zu ticks, %zu poses, status %s, map %zu, %.1f ms%s%s\n", sys.ticks_.size(), n_pose, sys.status_.c_str(), map.size(), wall_ms,

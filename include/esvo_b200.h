@@ -383,6 +383,44 @@ ESVO_API int esvo_stage_mapping_inputs_dev(esvo_ctx* ctx, const uint16_t* ex_dev
                                            const int64_t* pose_t_ns_dev, const double* poses_dev,
                                            size_t n_poses);
 ESVO_API int esvo_set_ts_pair_dev(esvo_ctx* ctx, const double T_world_left[16]);
+
+/* Device-resident hand-off of the closed loop: the time-surface history, the published local map and the tracker's
+ * reference cloud stay in HBM.  Results are bit for bit those of the host forms on host copies of the same data.
+ *
+ * replaces: esvo_Mapping::TS_history_ (esvo_Mapping.h, std::map<ros::Time, TimeSurfaceObservation>) as timeSurfaceCallback
+ * fills it (esvo_Mapping.cpp:716-762).  A ring of `capacity` stereo pairs on the device, keyed by build stamp.  capacity 0
+ * (the default) frees it; any call drops what the history held. */
+ESVO_API int esvo_ts_history_reserve_dev(esvo_ctx* ctx, size_t capacity);
+/* Stores the images of the last esvo_ts_build / esvo_run_ts_build of both cameras under stamp_ns: the device-to-device copy is
+ * ordered behind both builds with CUDA events, no host sync.  Like the map's operator[] followed by erase(begin()) while over
+ * capacity: a stored stamp is overwritten, and a full history drops its smallest stamp (or the new pair, if that is smaller).
+ * ESVO_ERR_STATE without a reserved history or before both cameras were built. */
+ESVO_API int esvo_ts_history_store_dev(esvo_ctx* ctx, int64_t stamp_ns);
+/* replaces: the TimeSurfaceObservation dataTransferring takes from TS_history_ (esvo_Mapping.cpp:494-533) handed to the mapper:
+ * the same effect as esvo_set_ts_pair with the two images stored under stamp_ns (SmoothTimeSurface included), so that
+ * esvo_bm_match / esvo_mapping_at_time / esvo_sgbm_compute(NULL, NULL) run on it.  A stamp that was never stored or has been
+ * dropped returns ESVO_ERR_STATE (esvo_last_error says which) and leaves the context as it was. */
+ESVO_API int esvo_set_ts_pair_stored_dev(esvo_ctx* ctx, int64_t stamp_ns, const double T_world_left[16]);
+/* replaces: publishPointCloud's packing (esvo_Mapping.cpp:909-953; the host form is frontend::packPointCloud over
+ * esvo_map_download): every DepthMap element, in element-list order, becomes p_world = R p_cam + t of T_world_result as f32
+ * x, y, z, into a device cloud the context keeps as "the cloud published at stamp_ns".  *n_points: the point count (0 for an
+ * empty map; the reference then publishes nothing).  Synchronises once, for the count. */
+ESVO_API int esvo_map_publish_dev(esvo_ctx* ctx, const double T_world_result[16], int64_t stamp_ns, size_t* n_points);
+/* Read-back of the published cloud into a device buffer of *n (in: capacity in points, out: count) x 3 floats, and its stamp
+ * (may be NULL); synchronous.  ESVO_ERR_STATE before the first publish, ESVO_ERR_CAPACITY (with *n set) if it does not fit. */
+ESVO_API int esvo_map_published_cloud_dev(esvo_ctx* ctx, float* xyz_dev, size_t* n, int64_t* stamp_ns);
+/* replaces: esvo_Tracking::refDataTransferring's copy of the reference cloud (esvo_Tracking.cpp:177-211): snapshots the newest
+ * cloud published on this context, which must be the one of stamp_ns (ESVO_ERR_STATE otherwise), for esvo_track_reset_dev;
+ * later publishes do not change it.  *n_points (may be NULL): its point count. */
+ESVO_API int esvo_track_adopt_map_dev(esvo_ctx* ctx, int64_t stamp_ns, size_t* n_points);
+/* replaces: RegProblemSolverLM::resetRegProblem -> RegProblemLM::setProblem (RegProblemSolverLM.cpp:45-74,
+ * RegProblemLM.cpp:24-68) on the adopted cloud: esvo_track_reset with the reference cloud on the device.  The stochastic
+ * sampling permutes an index list of the adopted cloud instead of the cloud, carried from reset to reset until the next
+ * adoption, with the same rand() draws (the stream esvo_track_reset and esvo_track_srand use); the result is exactly that of
+ * esvo_track_reset on a host copy of the cloud.  ts_left as in esvo_track_reset.  Returns 1 when the cloud has fewer than
+ * BATCH_SIZE points; ESVO_ERR_STATE before an adoption. */
+ESVO_API int esvo_track_reset_dev(esvo_ctx* ctx, const double T_world_ref[16], const double T_world_cur_prior[16],
+                                  const uint8_t* ts_left);
 /* Per-stage device timing with CUDA events on the ctx stream.  Stages: 0 time surface, 1 block
  * matching, 2 seed ordering, 3 depth LM, 4 point ordering/culling, 5 fusion+clean+regularise,
  * 6 tracking.  esvo_profile(ctx, stage_mask): bit s switches the timing of stage s on (0 = off, 0xff = all).

@@ -10,6 +10,7 @@
 #pragma once
 #include <algorithm>
 #include <array>
+#include <chrono>
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
@@ -62,9 +63,24 @@ struct TimeSurfaceObservation {
   const uint8_t* right = nullptr;
   Pose tr_{};
   size_t id_ = 0;
+  bool stored_ = false;             // the pair the device history holds under this observation's stamp (esvo_ts_history_store_dev)
   void setTransformation(const Pose& tr) { tr_ = tr; }
 };
 using StampedTimeSurfaceObs = std::pair<int64_t, TimeSurfaceObservation>;
+
+// Host time and call count per named call, accumulated over a run (scripts/loop_probe.py reports them).
+struct CallTimes {
+  struct Scope {
+    CallTimes* c; const char* name; std::chrono::steady_clock::time_point t0;
+    ~Scope() {
+      auto& e = c->ms[name];
+      e.first += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+      ++e.second;
+    }
+  };
+  Scope time(const char* name) { return Scope{this, name, std::chrono::steady_clock::now()}; }
+  std::map<std::string, std::pair<double, size_t>> ms;   // name -> (total ms, calls)
+};
 
 // Eigen::Quaterniond(const Matrix3d&) (Eigen/src/Geometry/Quaternion.h, quaternion_assign_impl): R row-major 3x3, q = x, y, z, w
 inline void quaternionFromRotation(const double R[9], double q[4]) {
@@ -310,8 +326,9 @@ class EventMatcher {
   std::vector<esvo::Event*>* pvCandEventPtr_ = nullptr;
 };
 
-// core::RefFrame / CurFrame (RegProblemLM.h:58-74)
-struct RefFrame { int64_t t_ = 0; std::vector<float> vPointXYZ_; /* n*3, world frame; permuted in place */ esvo::Pose tr_{}; };
+// core::RefFrame / CurFrame (RegProblemLM.h:58-74).  on_device_: the cloud is the one adopted on the device
+// (esvo_track_adopt_map_dev) instead of vPointXYZ_.
+struct RefFrame { int64_t t_ = 0; std::vector<float> vPointXYZ_; /* n*3, world frame; permuted in place */ esvo::Pose tr_{}; bool on_device_ = false; };
 struct CurFrame { int64_t t_ = 0; const uint8_t* ts_left = nullptr; esvo::Pose tr_{}; size_t numEventsSinceLastObs_ = 0; };
 struct LM_statics { size_t nPoints_ = 0, nfev_ = 0, nIter_ = 0; };
 enum RegProblemType { REG_NUMERICAL, REG_ANALYTICAL };
@@ -322,8 +339,9 @@ class RegProblemSolverLM {
   RegProblemSolverLM(CameraSystem::Ptr& camSysPtr, RegProblemType rpType = REG_ANALYTICAL) : camSysPtr_(camSysPtr), rpType_(rpType) {}
   bool resetRegProblem(RefFrame* ref, CurFrame* cur) {
     cur_ = cur;
-    int rc = esvo_track_reset(camSysPtr_->ctx(), ref->vPointXYZ_.data(), ref->vPointXYZ_.size() / 3, ref->tr_.data(),
-                              cur->tr_.data(), cur->ts_left);
+    int rc = ref->on_device_ ? esvo_track_reset_dev(camSysPtr_->ctx(), ref->tr_.data(), cur->tr_.data(), cur->ts_left)
+                             : esvo_track_reset(camSysPtr_->ctx(), ref->vPointXYZ_.data(), ref->vPointXYZ_.size() / 3, ref->tr_.data(),
+                                                cur->tr_.data(), cur->ts_left);
     lmStatics_ = LM_statics();
     return rc == ESVO_OK;   // 1 = not enough points in the local map -> the system re-initialises
   }
@@ -608,8 +626,7 @@ class esvo_Mapping {
   struct Counters { uint64_t n_events, n_seeds, n_solved, n_culled, n_fusions, bm_evals, lm_evals, map_size; };
   bool MappingAtTime(const esvo::StampedTimeSurfaceObs& TS_obs, const std::vector<esvo::Event*>& vCloseEventsPtr_left,
                      const esvo::StampTransformationMap& st_map, Counters* out = nullptr) {
-    const auto& obs = TS_obs.second;
-    if (esvo_set_ts_pair(cs_->ctx(), obs.left, obs.right, obs.tr_.data()) != ESVO_OK) return false;
+    if (!setObservation(TS_obs)) return false;
     std::vector<uint16_t> ex, ey; std::vector<int64_t> et, pt; std::vector<double> poses;
     for (auto* e : vCloseEventsPtr_left) { ex.push_back(e->x); ey.push_back(e->y); et.push_back(e->ts); }
     for (auto& st : st_map) { pt.push_back(st.first); poses.insert(poses.end(), st.second.begin(), st.second.end()); }
@@ -641,6 +658,7 @@ class esvo_Mapping {
                             size_t INIT_SGM_DP_NUM_Threshold, size_t* n_points = nullptr) {
     const int num_disparities = 16 * 3, block_size = 11;                       // esvo_Mapping.cpp:101-105
     std::vector<int16_t> disp((size_t)cs_->width_ * cs_->height_);
+    if (TS_obs.second.stored_ && !setObservation(TS_obs)) return false;      // a stored pair: the SGM reads the observation
     if (esvo_sgbm_compute(cs_->ctx(), TS_obs.second.left, TS_obs.second.right, num_disparities, block_size, 8 * block_size * block_size,
                           32 * block_size * block_size, -1, 0, 11, disp.data()) != ESVO_OK)
       return false;
@@ -674,8 +692,16 @@ class esvo_Mapping {
   void timeSurfaceCallback(int64_t stamp_ns, const uint8_t* time_surface_left, const uint8_t* time_surface_right) {
     const size_t n = (size_t)cs_->width_ * cs_->height_;
     TS_history_[stamp_ns] = TsPair{std::vector<uint8_t>(time_surface_left, time_surface_left + n),
-                                   std::vector<uint8_t>(time_surface_right, time_surface_right + n), TS_id_++};
+                                   std::vector<uint8_t>(time_surface_right, time_surface_right + n), TS_id_++, false};
     while (TS_history_.size() > TS_HISTORY_LENGTH_) TS_history_.erase(TS_history_.begin());
+  }
+  // Device form: the pair just built on this context (both cameras at stamp_ns) goes into the device history
+  // (esvo_ts_history_store_dev, reserved by the owner with TS_HISTORY_LENGTH_ pairs); the host history keeps the stamp only.
+  bool timeSurfaceCallback(int64_t stamp_ns) {
+    if (esvo_ts_history_store_dev(cs_->ctx(), stamp_ns) != ESVO_OK) return false;
+    TS_history_[stamp_ns] = TsPair{{}, {}, TS_id_++, true};
+    while (TS_history_.size() > TS_HISTORY_LENGTH_) TS_history_.erase(TS_history_.begin());
+    return true;
   }
   // dataTransferring (:494-605).  Leaves TS_obs_ (second-newest entry with a pose; identity in INITIALIZATION), and
   // vEventsPtr_left_SGM_ (INITIALIZATION) or vALLEventsPtr_left_ / vCloseEventsPtr_left_ / st_map_ (WORKING).
@@ -694,7 +720,9 @@ class esvo_Mapping {
       }
       if (has_obs_) {
         TS_obs_.first = it_end->first;
-        TS_obs_.second.left = it_end->second.left.data(); TS_obs_.second.right = it_end->second.right.data();
+        TS_obs_.second.stored_ = it_end->second.stored;
+        TS_obs_.second.left = it_end->second.stored ? nullptr : it_end->second.left.data();
+        TS_obs_.second.right = it_end->second.stored ? nullptr : it_end->second.right.data();
         TS_obs_.second.id_ = it_end->second.id; TS_obs_.second.setTransformation(tr);
       }
       if (it_end->first == t_oldest) break;
@@ -716,35 +744,40 @@ class esvo_Mapping {
     return true;
   }
   // What one pass of MappingLoop did.  ran: 0 nothing, 1 InitializationAtTime, 2 MappingAtTime; ok: the call's result;
-  // cloud: the local map as publishPointCloud publishes it (world frame, at the observation's pose), if it did.
+  // cloud: the local map as publishPointCloud publishes it (world frame, at the observation's pose), if it did; with a stored
+  // observation it is published on the device instead (esvo_map_publish_dev) and `cloud` stays empty.  cloud_points: its size.
   struct LoopResult {
     int ran = 0; bool ok = false; size_t n_sgm_points = 0; Counters ctr{};
-    bool published = false; int64_t stamp = 0; esvo::Pose T_world_obs{}; std::vector<float> cloud;
+    bool published = false; int64_t stamp = 0; esvo::Pose T_world_obs{}; std::vector<float> cloud; size_t cloud_points = 0;
   };
   // one pass of MappingLoop's body (:194-248) with publishMappingResults / publishPointCloud (:396-403,488-490,868-953) run in line
   bool MappingLoopOnce(LoopResult& res) {
     res = LoopResult();
     if (ESVO_System_Status_ == "TERMINATE" || TS_history_.size() < 10) return false;
-    dataTransferring();
+    { auto _ = calls_.time("mapping.dataTransferring"); dataTransferring(); }
     if (!has_obs_) return false;
     if (ESVO_System_Status_ == "INITIALIZATION" || ESVO_System_Status_ == "RESET") {
       res.ran = 1;
-      res.ok = InitializationAtTime(TS_obs_, vEventsPtr_left_SGM_, INIT_SGM_DP_NUM_Threshold_, &res.n_sgm_points);
-      if (res.ok) publishMappingResults(res);
+      { auto _ = calls_.time("mapping.InitializationAtTime");
+        res.ok = InitializationAtTime(TS_obs_, vEventsPtr_left_SGM_, INIT_SGM_DP_NUM_Threshold_, &res.n_sgm_points); }
+      if (res.ok) { auto _ = calls_.time("mapping.publishMappingResults"); publishMappingResults(res); }
     }
     if (ESVO_System_Status_ == "WORKING") {
       res.ran = 2;
-      vDenoisedEventsPtr_left_.clear();
-      if (bDenoising_) {                                   // :282-296
-        std::vector<uint8_t> mask;
-        frontend::createDenoisingMask(vALLEventsPtr_left_, mask, (size_t)cs_->height_, (size_t)cs_->width_);
-        frontend::extractDenoisedEvents(vCloseEventsPtr_left_, vDenoisedEventsPtr_left_, mask, (size_t)cs_->width_, PROCESS_EVENT_NUM_);
-      } else {                                             // :297-304
-        vDenoisedEventsPtr_left_.assign(vCloseEventsPtr_left_.begin(),
-                                        vCloseEventsPtr_left_.begin() + (long)std::min(vCloseEventsPtr_left_.size(), PROCESS_EVENT_NUM_));
+      {
+        auto _ = calls_.time("mapping.denoising");
+        vDenoisedEventsPtr_left_.clear();
+        if (bDenoising_) {                                   // :282-296
+          std::vector<uint8_t> mask;
+          frontend::createDenoisingMask(vALLEventsPtr_left_, mask, (size_t)cs_->height_, (size_t)cs_->width_);
+          frontend::extractDenoisedEvents(vCloseEventsPtr_left_, vDenoisedEventsPtr_left_, mask, (size_t)cs_->width_, PROCESS_EVENT_NUM_);
+        } else {                                             // :297-304
+          vDenoisedEventsPtr_left_.assign(vCloseEventsPtr_left_.begin(),
+                                          vCloseEventsPtr_left_.begin() + (long)std::min(vCloseEventsPtr_left_.size(), PROCESS_EVENT_NUM_));
+        }
       }
-      res.ok = MappingAtTime(TS_obs_, vDenoisedEventsPtr_left_, st_map_, &res.ctr);
-      if (res.ok) publishMappingResults(res);
+      { auto _ = calls_.time("mapping.MappingAtTime"); res.ok = MappingAtTime(TS_obs_, vDenoisedEventsPtr_left_, st_map_, &res.ctr); }
+      if (res.ok) { auto _ = calls_.time("mapping.publishMappingResults"); publishMappingResults(res); }
     }
     return res.ok;
   }
@@ -763,7 +796,14 @@ class esvo_Mapping {
   esvo::StampedTimeSurfaceObs TS_obs_;
   std::vector<esvo::Event*> vEventsPtr_left_SGM_, vALLEventsPtr_left_, vCloseEventsPtr_left_, vDenoisedEventsPtr_left_;
   esvo::StampTransformationMap st_map_;
+  esvo::CallTimes calls_;   // host time of each call MappingLoopOnce makes
  private:
+  // the observation to the device: the stored pair by its stamp, or the host images (nullptr: the last builds)
+  bool setObservation(const esvo::StampedTimeSurfaceObs& TS_obs) {
+    const auto& obs = TS_obs.second;
+    if (obs.stored_) return esvo_set_ts_pair_stored_dev(cs_->ctx(), TS_obs.first, obs.tr_.data()) == ESVO_OK;
+    return esvo_set_ts_pair(cs_->ctx(), obs.left, obs.right, obs.tr_.data()) == ESVO_OK;
+  }
   // publishMappingResults (:868-907): in INITIALIZATION always, in WORKING once the fusion window is full (CONST_FRAMES) or
   // holds more than half of maxNumFusionPoints (CONST_POINTS); publishPointCloud (:909-953) skips an empty cloud
   void publishMappingResults(LoopResult& res) {
@@ -776,15 +816,20 @@ class esvo_Mapping {
       else publish = (double)n_points > 0.5 * (double)p.max_num_fusion_points;
     }
     if (!publish) return;
-    std::vector<esvo::DepthPoint> elems((size_t)cs_->width_ * cs_->height_);
-    size_t n = elems.size();
-    if (esvo_map_download(cs_->ctx(), elems.data(), &n) != ESVO_OK) n = 0;
-    elems.resize(n);
-    frontend::packPointCloud(elems, TS_obs_.second.tr_, res.cloud);
-    if (res.cloud.empty()) return;
+    if (TS_obs_.second.stored_) {                        // device form: the cloud stays on the device for the tracker
+      if (esvo_map_publish_dev(cs_->ctx(), TS_obs_.second.tr_.data(), TS_obs_.first, &res.cloud_points) != ESVO_OK) res.cloud_points = 0;
+    } else {
+      std::vector<esvo::DepthPoint> elems((size_t)cs_->width_ * cs_->height_);
+      size_t n = elems.size();
+      if (esvo_map_download(cs_->ctx(), elems.data(), &n) != ESVO_OK) n = 0;
+      elems.resize(n);
+      frontend::packPointCloud(elems, TS_obs_.second.tr_, res.cloud);
+      res.cloud_points = res.cloud.size() / 3;
+    }
+    if (res.cloud_points == 0) return;
     res.published = true; res.stamp = TS_obs_.first; res.T_world_obs = TS_obs_.second.tr_;
   }
-  struct TsPair { std::vector<uint8_t> left, right; size_t id; };
+  struct TsPair { std::vector<uint8_t> left, right; size_t id; bool stored; };   // stored: the images are in the device history
   esvo::CameraSystem::Ptr cs_;
   std::deque<esvo::Event> events_left_, events_right_;   // EventQueue (esvo_Mapping.h)
   std::map<int64_t, TsPair> TS_history_;
@@ -1199,13 +1244,25 @@ class esvo_Tracking {
   // refMapCallback: the local map as the mapping node publishes it (pcl::PointXYZ: f32 x,y,z in the WORLD frame, i.e. the
   // output of frontend::packPointCloud); at most REF_HISTORY_LENGTH maps are kept.
   void refMapCallback(int64_t stamp_ns, const std::vector<float>& xyz) {
-    refPCMap_[stamp_ns] = std::make_shared<std::vector<float>>(xyz);
+    refPCMap_[stamp_ns] = RefMap{std::make_shared<std::vector<float>>(xyz), xyz.size() / 3};
+    while (refPCMap_.size() > REF_HISTORY_LENGTH_) refPCMap_.erase(refPCMap_.begin());
+  }
+  // Device form: the cloud of n_points the mapper published on this context at stamp_ns (esvo_map_publish_dev); it stays
+  // there, and refDataTransferring adopts it (esvo_track_adopt_map_dev).
+  void refMapCallback(int64_t stamp_ns, size_t n_points) {
+    refPCMap_[stamp_ns] = RefMap{nullptr, n_points};
     while (refPCMap_.size() > REF_HISTORY_LENGTH_) refPCMap_.erase(refPCMap_.begin());
   }
   // timeSurfaceCallback: mono8 left image (H*W); the tracker only reads the left one (:331-349).
   void timeSurfaceCallback(int64_t stamp_ns, const uint8_t* time_surface_left) {
     const size_t n = (size_t)cs_->width_ * cs_->height_;
     TS_history_[stamp_ns] = TsEntry{std::vector<uint8_t>(time_surface_left, time_surface_left + n), TS_id_++};
+    while (TS_history_.size() > TS_HISTORY_LENGTH_) TS_history_.erase(TS_history_.begin());
+  }
+  // Device form: the left image just built on this context at stamp_ns; the history keeps the stamp, and the registration
+  // reads the newest camera-0 build (esvo_track_reset with ts_left = NULL).
+  void timeSurfaceCallback(int64_t stamp_ns) {
+    TS_history_[stamp_ns] = TsEntry{{}, TS_id_++};
     while (TS_history_.size() > TS_HISTORY_LENGTH_) TS_history_.erase(TS_history_.begin());
   }
   // eventsCallback: insertion-sorted event buffer, capped at 5e6 (:294-321)
@@ -1227,7 +1284,13 @@ class esvo_Tracking {
     if (ESVO_System_Status_ == "WORKING" || (ESVO_System_Status_ == "INITIALIZATION" && ets_ == WORKING)) {
       if (!getPoseAt_ || !getPoseAt_(ref_.t_, ref_.tr_)) return false;   // the reference exit(-1)s here ("logic error")
     }
-    ref_.vPointXYZ_ = *refPCMap_.rbegin()->second;    // the reference keeps pointers into the cloud; the device path permutes a copy
+    const RefMap& m = refPCMap_.rbegin()->second;
+    ref_.on_device_ = !m.host;
+    if (m.host) ref_.vPointXYZ_ = *m.host;             // the reference keeps pointers into the cloud; the device path permutes a copy
+    else {
+      ref_.vPointXYZ_.clear();
+      if (esvo_track_adopt_map_dev(cs_->ctx(), ref_.t_, nullptr) != ESVO_OK) { error_ = std::string("adopting the map: ") + esvo_last_error(cs_->ctx()); return false; }
+    }
     return true;
   }
   // ---- curDataTransferring (:213-245) ----
@@ -1236,7 +1299,7 @@ class esvo_Tracking {
     auto TS_it = TS_history_.rbegin();
     if (cur_.t_ == TS_it->first) return false;        // TS_history may not have been updated yet
     cur_.t_ = TS_it->first;
-    cur_.ts_left = TS_it->second.left.data();
+    cur_.ts_left = TS_it->second.left.empty() ? nullptr : TS_it->second.left.data();   // empty: the newest camera-0 build
     if (ESVO_System_Status_ == "INITIALIZATION" && ets_ == IDLE) cur_.tr_ = ref_.tr_;
     if (ESVO_System_Status_ == "WORKING" || (ESVO_System_Status_ == "INITIALIZATION" && ets_ == WORKING)) cur_.tr_ = T_world_cur_;
     const size_t ev_cur = lower_bound_ev(cur_.t_);
@@ -1249,7 +1312,7 @@ class esvo_Tracking {
     if (ESVO_System_Status_ == "INITIALIZATION" && ets_ == WORKING) { reset(); return false; }
     if (ESVO_System_Status_ == "TERMINATE") return false;
     if (frontend::toSec(ref_.t_) < frontend::toSec(refPCMap_.rbegin()->first))            // new reference map arrived
-      if (!refDataTransferring()) { error_ = "no pose for the reference map"; return false; }
+      if (!refDataTransferring()) { if (error_.empty()) error_ = "no pose for the reference map"; return false; }
     if (frontend::toSec(cur_.t_) < frontend::toSec(TS_history_.rbegin()->first)) {          // new observation arrived
       if (frontend::toSec(ref_.t_) >= frontend::toSec(TS_history_.rbegin()->first)) {       // obs must come after the ref (reference: exit(-1))
         error_ = "time-surface observation is not newer than the reference map";
@@ -1311,7 +1374,8 @@ class esvo_Tracking {
   esvo::CameraSystem::Ptr cs_;
   core::RegProblemType rpType_;
   size_t TS_HISTORY_LENGTH_, REF_HISTORY_LENGTH_, TS_id_ = 0;
-  std::map<int64_t, std::shared_ptr<std::vector<float>>> refPCMap_;
+  struct RefMap { std::shared_ptr<std::vector<float>> host; size_t n; };   // host == nullptr: published on the device
+  std::map<int64_t, RefMap> refPCMap_;
   std::map<int64_t, TsEntry> TS_history_;
   std::deque<esvo::Event> events_left_;
   PoseProvider getPoseAt_;

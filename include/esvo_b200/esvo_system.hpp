@@ -6,11 +6,13 @@
 // t_k = t0 + k * dt (DESIGN.md section 5):
 //   1. every event with stamp < t_k that has not been delivered goes to both time surfaces, the mapper's left / right
 //      buffers and the tracker's left buffer;
-//   2. both time surfaces are built at t_k; the pair goes to the mapper's history, the left image to the tracker's;
+//   2. both time surfaces are built at t_k; the pair goes to the mapper's history, the left image to the tracker's -- on the
+//      device: the mapper's history is the context's time-surface history, the tracker reads the newest camera-0 build;
 //   3. esvo_Tracking::TrackingLoopOnce(); a pose it produces goes into the pose buffer at once (publishPose ->
 //      stampedPoseCallback);
 //   4. every mapping_every-th tick esvo_Mapping::MappingLoopOnce(); a map it publishes goes to the tracker's
-//      refMapCallback with the map's stamp.
+//      refMapCallback with the map's stamp -- published and adopted on the device (esvo_map_publish_dev,
+//      esvo_track_adopt_map_dev), never downloaded.
 // Where a reference node calls exit(-1) the system sets the status to TERMINATE, keeps the reason in error_ and stops.
 // Header-only; link with libesvo_b200.so.
 #pragma once
@@ -42,8 +44,7 @@ class esvo_System {
   };
 
   esvo_System(esvo::CameraSystem::Ptr cs, const Config& cfg)
-      : cfg_(cfg), cs_(cs), ts_left_(cs, 0), ts_right_(cs, 1), mapper_(cs), tracker_(cs, cfg.rpType, cfg.TRK_TS_HISTORY_LENGTH, cfg.REF_HISTORY_LENGTH),
-        img_l_((size_t)cs->width_ * cs->height_), img_r_((size_t)cs->width_ * cs->height_) {
+      : cfg_(cfg), cs_(cs), ts_left_(cs, 0), ts_right_(cs, 1), mapper_(cs), tracker_(cs, cfg.rpType, cfg.TRK_TS_HISTORY_LENGTH, cfg.REF_HISTORY_LENGTH) {
     mapper_.PROCESS_EVENT_NUM_ = cfg.PROCESS_EVENT_NUM; mapper_.TS_HISTORY_LENGTH_ = cfg.TS_HISTORY_LENGTH;
     mapper_.INIT_SGM_DP_NUM_Threshold_ = cfg.INIT_SGM_DP_NUM_THRESHOLD; mapper_.BM_half_slice_thickness_ = cfg.BM_half_slice_thickness;
     mapper_.bDenoising_ = cfg.Denoising;
@@ -51,6 +52,8 @@ class esvo_System {
     mapper_.setPoseProvider(poseAt);
     tracker_.setPoseProvider(poseAt);
     esvo_track_srand(cs->ctx(), 1);        // the reference never seeds rand(): glibc seed 1
+    if (esvo_ts_history_reserve_dev(cs->ctx(), cfg.TS_HISTORY_LENGTH) != ESVO_OK)
+      throw std::runtime_error(std::string("esvo_ts_history_reserve_dev: ") + esvo_last_error(cs->ctx()));
   }
   int64_t nextTick() const { return cfg_.t0_ns + (int64_t)k_ * cfg_.dt_ns; }
   // One sync tick.  left / right: the events with stamp < nextTick() not delivered yet, time-ordered.  false once stopped.
@@ -61,16 +64,19 @@ class esvo_System {
     TickRecord rec;
     rec.t = nextTick();
     const auto c0 = clk::now();
-    bool ok = (left.empty() || ts_left_.eventsCallback(left)) && (right.empty() || ts_right_.eventsCallback(right));
-    mapper_.eventsCallback(left, true); mapper_.eventsCallback(right, false);
-    tracker_.eventsCallback(left);
-    ok = ok && ts_left_.createTimeSurfaceAtTime(rec.t, img_l_.data()) && ts_right_.createTimeSurfaceAtTime(rec.t, img_r_.data());
+    bool ok;
+    { auto _ = calls_.time("ts.eventsCallback"); ok = (left.empty() || ts_left_.eventsCallback(left)) && (right.empty() || ts_right_.eventsCallback(right)); }
+    { auto _ = calls_.time("mapping.eventsCallback"); mapper_.eventsCallback(left, true); mapper_.eventsCallback(right, false); }
+    { auto _ = calls_.time("tracking.eventsCallback"); tracker_.eventsCallback(left); }
+    { auto _ = calls_.time("ts.createTimeSurfaceAtTime");
+      ok = ok && ts_left_.createTimeSurfaceAtTime(rec.t, nullptr) && ts_right_.createTimeSurfaceAtTime(rec.t, nullptr); }
     if (!ok) return stop(std::string("time surface: ") + esvo_last_error(cs_->ctx()), rec);
-    mapper_.timeSurfaceCallback(rec.t, img_l_.data(), img_r_.data());
-    tracker_.timeSurfaceCallback(rec.t, img_l_.data());
+    { auto _ = calls_.time("mapping.timeSurfaceCallback");
+      if (!mapper_.timeSurfaceCallback(rec.t)) return stop(std::string("time-surface history: ") + esvo_last_error(cs_->ctx()), rec); }
+    { auto _ = calls_.time("tracking.timeSurfaceCallback"); tracker_.timeSurfaceCallback(rec.t); }
     const auto c1 = clk::now();
     tracker_.ESVO_System_Status_ = status_;
-    rec.has_pose = tracker_.TrackingLoopOnce();
+    { auto _ = calls_.time("tracking.TrackingLoopOnce"); rec.has_pose = tracker_.TrackingLoopOnce(); }
     status_ = tracker_.ESVO_System_Status_;
     if (!tracker_.error_.empty()) return stop("tracking: " + tracker_.error_, rec);
     if (rec.has_pose) { rec.T = tracker_.T_world_cur_; poses_.setTransform(tracker_.cur_.t_, tracker_.cur_.tr_); }
@@ -78,12 +84,12 @@ class esvo_System {
     if (k_ % (size_t)cfg_.mapping_every == 0) {
       mapper_.ESVO_System_Status_ = status_;
       esvo_Mapping::LoopResult r;
-      mapper_.MappingLoopOnce(r);
+      { auto _ = calls_.time("mapping.MappingLoopOnce"); mapper_.MappingLoopOnce(r); }
       status_ = mapper_.ESVO_System_Status_;
       MappingRecord m;
       m.tick = k_; m.ran = r.ran; m.ok = r.ok; m.n_sgm_points = r.n_sgm_points; m.ctr = r.ctr;
-      m.published = r.published; m.cloud_points = r.cloud.size() / 3; m.stamp = r.stamp;
-      if (r.published) tracker_.refMapCallback(r.stamp, r.cloud);
+      m.published = r.published; m.cloud_points = r.cloud_points; m.stamp = r.stamp;
+      if (r.published) tracker_.refMapCallback(r.stamp, r.cloud_points);
       mapping_.push_back(m);
     }
     const auto c3 = clk::now();
@@ -96,6 +102,12 @@ class esvo_System {
   // the fused map the mapper holds (DepthMap element order)
   void getMap(std::vector<esvo::DepthPoint>& out) { core::DepthFusion f(cs_); f.getElements(out); }
   bool saveTrajectory(const std::string& path) const { return tracker_.saveTrajectory(path); }
+  // host time of each call SpinOnce makes, and of each call MappingLoopOnce makes (names "mapping.*" inside it)
+  esvo::CallTimes callTimes() const {
+    esvo::CallTimes all = calls_;
+    for (const auto& e : mapper_.calls_.ms) all.ms[e.first] = e.second;
+    return all;
+  }
 
   const Config& config() const { return cfg_; }
   std::string status_ = "INITIALIZATION";   // /ESVO_SYSTEM_STATUS
@@ -115,7 +127,7 @@ class esvo_System {
   esvo_time_surface::TimeSurface ts_left_, ts_right_;
   esvo_Mapping mapper_;
   esvo_Tracking tracker_;
-  std::vector<uint8_t> img_l_, img_r_;
+  esvo::CallTimes calls_;
   size_t k_ = 0;
 };
 

@@ -1,8 +1,12 @@
 """Measures the closed loop (examples/system_loop.cpp, esvo_core::esvo_System) on a seeded 2 s hkust stream and prints one
 JSON line: the card and its power limit, wall time per second of stream, mapping / tracking / time-surface ms, the per-stage
-esvo_profile breakdown, when tracking starts, how well it follows the ground truth, and the same stream through the Python
-restatement (tests/indep_system.py) on the CPU oracle.  Builds the example into a temporary directory; writes nothing in the
-tree.  usage: python scripts/loop_probe.py [--seconds 2.0] [--seed 2] [--no-oracle]"""
+esvo_profile breakdown, the host time of every call SpinOnce and MappingLoopOnce make (ms per tick or per mapping frame that
+made the call), when tracking starts, how well it follows the ground truth, and the same stream through the Python
+restatement (tests/indep_system.py) on the CPU oracle.  Scenes as in tests/test_system_loop.py: "dense" (the default
+80-segment scene) and "mapping" (7 segments at 0.5-1.2 m, twice the speed: WORKING maps are published and adopted).
+--root: the tree whose library and example are measured (default: this one), to compare builds in one session.
+Builds the example into a temporary directory; writes nothing in the tree.
+usage: python scripts/loop_probe.py [--seconds 2.0] [--seed 2] [--scene dense|mapping] [--root DIR] [--no-oracle]"""
 import argparse
 import json
 import os
@@ -17,6 +21,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 DT_NS = 10_000_000
+SCENES = {"dense": (dict(), 1.0), "mapping": (dict(n_segments=7, speed=2.0, depth_range=(0.5, 1.2)), 2.0)}
 STAGES = ["time_surface", "block_matching", "seed_ordering", "depth_lm", "point_ordering_culling", "fusion_clean_regularise", "tracking", "stage7"]
 
 
@@ -30,26 +35,37 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--seconds", type=float, default=2.0)
     ap.add_argument("--seed", type=int, default=2)
+    ap.add_argument("--scene", choices=list(SCENES), default="dense")
+    ap.add_argument("--root", default=ROOT)
     ap.add_argument("--no-oracle", action="store_true")
     a = ap.parse_args()
     import indep_system as isy
     from esvo_b200 import synth
-    s = synth.make_stream("hkust", seed=a.seed, t_ts=a.seconds, history_ms=a.seconds * 1e3)
+    kw, speed = SCENES[a.scene]
+    s = synth.make_stream("hkust", seed=a.seed, t_ts=a.seconds, history_ms=a.seconds * 1e3, **kw)
     t0 = s["t_ts_ns"] - int(round(a.seconds * 1e9)) + DT_NS
     n = int(round(a.seconds * 1e9 / DT_NS))
-    gt = lambda t: synth.pose_at(t * 1e-9)
-    out = {"workload": f"hkust synthetic stream, seed {a.seed}, {a.seconds:g} s, {n} ticks at 100 Hz, mapping at 20 Hz, hkust yaml"}
+    gt = lambda t: synth.pose_at(t * 1e-9 * speed)
+    out = {"workload": f"hkust synthetic stream, {a.scene} scene, seed {a.seed}, {a.seconds:g} s, {n} ticks at 100 Hz, mapping at 20 Hz, "
+                       f"hkust yaml", "root": os.path.abspath(a.root)}
     out["gpu"], out["power_limit"] = card()
     with tempfile.TemporaryDirectory() as tmp:
-        build = os.path.join(ROOT, "esvo_b200", "_build")
+        build = os.path.join(a.root, "esvo_b200", "_build")
         exe = os.path.join(tmp, "system_loop")
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + os.path.join(ROOT, "include"), os.path.join(ROOT, "examples", "system_loop.cpp"),
+        subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + os.path.join(a.root, "include"), os.path.join(a.root, "examples", "system_loop.cpp"),
                                "-L" + build, "-lesvo_b200", "-Wl,-rpath," + build, "-o", exe])
         isy.write_scenario(os.path.join(tmp, "s.bin"), 346, 260, t0, DT_NS, n, s["left"], s["right"], profile=True)
-        p = subprocess.run([exe, os.path.join(tmp, "s.bin"), os.path.join(tmp, "r.bin"), os.path.join(tmp, "t.txt")], capture_output=True, text=True)
+        calls_path = os.path.join(tmp, "calls.txt")
+        p = subprocess.run([exe, os.path.join(tmp, "s.bin"), os.path.join(tmp, "r.bin"), os.path.join(tmp, "t.txt"), calls_path],
+                           capture_output=True, text=True)
         if p.returncode:
             raise SystemExit(p.stdout + p.stderr)
         ticks, maps, m, stopped, wall, prof_ms, prof_n = isy.parse_result(os.path.join(tmp, "r.bin"))
+        calls = {}
+        if os.path.exists(calls_path):            # a tree whose example writes no call times has no breakdown
+            for line in open(calls_path):
+                name, total, count = line.split()
+                calls[name] = {"ms_per_call": round(float(total) / max(int(count), 1), 4), "calls": int(count)}
     ms = ticks["ms"]
     mapped = np.isin(np.arange(ticks.size), maps[maps["ran"] == 2]["tick"])
     posed = ticks["has_pose"] == 1
@@ -61,6 +77,7 @@ def main():
     out["ts_ms_per_tick"] = {"median": q(ms[:, 0], 50), "p90": q(ms[:, 0], 90)}
     out["profile_ms"] = {STAGES[i]: round(float(prof_ms[i]), 3) for i in range(8) if prof_n[i]}
     out["profile_launches"] = {STAGES[i]: int(prof_n[i]) for i in range(8) if prof_n[i]}
+    out["host_ms_per_call"] = calls
     out["first_pose_tick"] = int(np.argmax(posed)) if posed.any() else None
     out["tracked_frames"] = int(posed.sum())
     out["stopped"] = bool(stopped)
