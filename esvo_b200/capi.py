@@ -435,6 +435,54 @@ class Backend:
                    C.byref(n), C.byref(acc))
         return int(n.value), bool(acc.value)
 
+    # ---- event windows read from the time-surface log (product only) ----
+    def events_window_dev(self, cam, front, t_begin_ns, t_end_ns, budget, denoise, max_keep, ok=(0,)):
+        """esvo_events_window_dev: returns (rc, size of the selection); rc in ok, else EsvoError."""
+        n = C.c_size_t(0)
+        rc = self._call("events_window_dev", [C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_size_t, C.c_int, C.c_size_t, C.POINTER(C.c_size_t)],
+                        int(cam), int(front), int(t_begin_ns), int(t_end_ns), int(budget), int(bool(denoise)), int(max_keep), C.byref(n), ok=ok)
+        return rc, int(n.value)
+
+    def events_lower_bound_dev(self, cam, front, t_ns, ok=(0,)):
+        """esvo_events_lower_bound_dev: returns (rc, global push indices)."""
+        t = _arr(t_ns, np.int64)
+        out = np.zeros(t.size, np.int64)
+        rc = self._call("events_lower_bound_dev", [C.c_int, C.c_int64, C.POINTER(C.c_int64), C.c_size_t, C.POINTER(C.c_int64)],
+                        int(cam), int(front), _ptr(t, C.c_int64), t.size, _ptr(out, C.c_int64), ok=ok)
+        return rc, out
+
+    def events_selected_dev(self):
+        """The last selection (x, y, t, newest first), read back through device buffers."""
+        import torch
+        cap = max(int(self.evw_cap) if hasattr(self, "evw_cap") else 0, 1)
+        while True:
+            x = torch.zeros(cap, dtype=torch.int16, device="cuda"); y = torch.zeros(cap, dtype=torch.int16, device="cuda")
+            t = torch.zeros(cap, dtype=torch.int64, device="cuda")
+            n = C.c_size_t(cap)
+            rc = self._call("events_selected_dev", [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)], C.c_void_p(x.data_ptr()),
+                            C.c_void_p(y.data_ptr()), C.c_void_p(t.data_ptr()), C.byref(n), ok=(0, -4))
+            if rc == 0:
+                k = int(n.value)
+                return (x[:k].cpu().numpy().view(np.uint16), y[:k].cpu().numpy().view(np.uint16), t[:k].cpu().numpy())
+            cap = int(n.value); self.evw_cap = cap
+
+    def mapping_at_time_selected_dev(self, pose_t, poses):
+        pt = _arr(pose_t, np.int64); ps = _arr(poses, np.float64)
+        ctr = (C.c_uint64 * 8)()
+        self._call("mapping_at_time_selected_dev", [C.POINTER(C.c_int64), C.POINTER(C.c_double), C.c_size_t, C.POINTER(C.c_uint64)],
+                   _ptr(pt, C.c_int64), _ptr(ps, C.c_double), pt.size, ctr)
+        keys = ["n_events", "n_seeds", "n_solved", "n_culled", "n_fusions", "bm_evals", "lm_evals", "map_size"]
+        return dict(zip(keys, [int(v) for v in ctr]))
+
+    def init_from_disparity_selected_dev(self, disp16, T_world_left, min_points):
+        d = _arr(disp16, np.int16); T = np.ascontiguousarray(T_world_left, np.float64)
+        assert d.size == self.W * self.H
+        n = C.c_size_t(0); acc = C.c_int(0)
+        self._call("init_from_disparity_selected_dev", [C.POINTER(C.c_int16), C.POINTER(C.c_double), C.c_size_t, C.POINTER(C.c_size_t),
+                                                        C.POINTER(C.c_int)],
+                   _ptr(d, C.c_int16), _ptr(T, C.c_double), int(min_points), C.byref(n), C.byref(acc))
+        return int(n.value), bool(acc.value)
+
     def ts_set_unordered_input(self, cam, enable):
         self._call("ts_set_unordered_input", [C.c_int, C.c_int], int(cam), int(bool(enable)))
 

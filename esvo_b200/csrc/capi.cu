@@ -352,6 +352,7 @@ ESVO_API void esvo_destroy(esvo_ctx* c) {
   for (int cam = 0; cam < 2; ++cam) ts_free(c, cam);
   for (int i = 0; i < kMaxSlots; ++i) if (c->slots[i].map) { c->map = c->slots[i].map; fuse_free(c); c->slots[i].map = nullptr; }
   track_free(c);
+  ew_free(c);
   if (c->d_lut) cudaFree(c->d_lut);
   if (c->d_mask) cudaFree(c->d_mask);
   for (int i = 0; i < kMaxSlots; ++i) {

@@ -307,10 +307,12 @@ ESVO_API int esvo_sgbm_compute(esvo_ctx* c, const uint8_t* left, const uint8_t* 
   return rc;
 }
 
-ESVO_API int esvo_init_from_disparity(esvo_ctx* c, const int16_t* disp16, const uint16_t* ex, const uint16_t* ey, size_t n,
-                                      const double T[16], size_t min_points, size_t* n_points, int* accepted) {
-  CHECK_CTX(c);
-  if (!disp16 || !T || (n && (!ex || !ey))) return ESVO_ERR_INVALID_ARG;
+}  // extern "C"
+
+// InitializationAtTime downstream of the SGM (esvo_Mapping.cpp:433-492) on events that are on the device already (ex_dev / ey_dev),
+// or, with ex / ey, on host events uploaded first.
+static int init_from_disparity(esvo_ctx* c, const int16_t* disp16, const uint16_t* ex, const uint16_t* ey, const uint16_t* ex_dev,
+                               const uint16_t* ey_dev, size_t n, const double T[16], size_t min_points, size_t* n_points, int* accepted) {
   { int rc0 = drain(c); if (rc0) return rc0; }                     // a one-off at start-up: strictly synchronous
   const size_t npix = (size_t)c->dc.W * c->dc.H;
   int16_t* d_disp = nullptr; uint16_t *d_x = nullptr, *d_y = nullptr;
@@ -318,13 +320,15 @@ ESVO_API int esvo_init_from_disparity(esvo_ctx* c, const int16_t* disp16, const 
   int rc = win_acquire(c, std::max<size_t>(n, 1), f);
   if (rc) return rc;
   auto cleanup = [&]() { cudaFree(d_disp); cudaFree(d_x); cudaFree(d_y); };
-  if (dmalloc(&d_disp, npix) || dmalloc(&d_x, n) || dmalloc(&d_y, n)) { cleanup(); c->win_pool.push_back(f); return ESVO_ERR_CUDA; }
+  if (dmalloc(&d_disp, npix) || (!ex_dev && (dmalloc(&d_x, n) || dmalloc(&d_y, n)))) { cleanup(); c->win_pool.push_back(f); return ESVO_ERR_CUDA; }
   cudaError_t ce = cudaMemcpyAsync(d_disp, disp16, npix * 2, cudaMemcpyHostToDevice, c->stream);
-  if (n && ce == cudaSuccess) ce = cudaMemcpyAsync(d_x, ex, n * 2, cudaMemcpyHostToDevice, c->stream);
-  if (n && ce == cudaSuccess) ce = cudaMemcpyAsync(d_y, ey, n * 2, cudaMemcpyHostToDevice, c->stream);
+  if (!ex_dev && n && ce == cudaSuccess) ce = cudaMemcpyAsync(d_x, ex, n * 2, cudaMemcpyHostToDevice, c->stream);
+  if (!ex_dev && n && ce == cudaSuccess) ce = cudaMemcpyAsync(d_y, ey, n * 2, cudaMemcpyHostToDevice, c->stream);
   if (ce != cudaSuccess) { cleanup(); c->win_pool.push_back(f); c->set_error(cudaGetErrorString(ce)); return ESVO_ERR_CUDA; }
   unsigned long long cnt = 0;
-  if ((rc = fuse_reset_map(c, T)) == ESVO_OK && (rc = sgm_points(c, d_disp, d_x, d_y, n, f.pts, f.cnt)) == ESVO_OK) {
+  const uint16_t* px = ex_dev ? ex_dev : d_x;
+  const uint16_t* py = ex_dev ? ey_dev : d_y;
+  if ((rc = fuse_reset_map(c, T)) == ESVO_OK && (rc = sgm_points(c, d_disp, px, py, n, f.pts, f.cnt)) == ESVO_OK) {
     if (cudaMemcpyAsync(&cnt, f.cnt, 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess)
       rc = ESVO_ERR_CUDA;
   }
@@ -345,6 +349,70 @@ ESVO_API int esvo_init_from_disparity(esvo_ctx* c, const int16_t* disp16, const 
   ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   if (accepted) *accepted = 1;
   return ESVO_OK;
+}
+
+extern "C" {
+
+ESVO_API int esvo_init_from_disparity(esvo_ctx* c, const int16_t* disp16, const uint16_t* ex, const uint16_t* ey, size_t n,
+                                      const double T[16], size_t min_points, size_t* n_points, int* accepted) {
+  CHECK_CTX(c);
+  if (!disp16 || !T || (n && (!ex || !ey))) return ESVO_ERR_INVALID_ARG;
+  return init_from_disparity(c, disp16, ex, ey, nullptr, nullptr, n, T, min_points, n_points, accepted);
+}
+
+// ---- event windows read from the time-surface log (events.cu) ----
+ESVO_API int esvo_events_window_dev(esvo_ctx* c, int cam, int64_t front, int64_t t_begin_ns, int64_t t_end_ns, size_t budget, int denoise,
+                                    size_t max_keep, size_t* n) {
+  CHECK_CTX(c);
+  if (cam < 0 || cam > 1) return ESVO_ERR_INVALID_ARG;
+  return events_window(c, cam, front, t_begin_ns, t_end_ns, budget, denoise, max_keep, n);
+}
+ESVO_API int esvo_events_lower_bound_dev(esvo_ctx* c, int cam, int64_t front, const int64_t* t_ns, size_t k, int64_t* idx_out) {
+  CHECK_CTX(c);
+  if (cam < 0 || cam > 1 || (k && (!t_ns || !idx_out))) return ESVO_ERR_INVALID_ARG;
+  return events_lower_bound(c, cam, front, t_ns, k, idx_out);
+}
+ESVO_API int esvo_events_selected_dev(esvo_ctx* c, uint16_t* x_dev, uint16_t* y_dev, int64_t* t_dev, size_t* n) {
+  CHECK_CTX(c);
+  if (!n) return ESVO_ERR_INVALID_ARG;
+  const Ctx::EventWindow& w = c->evw;
+  if (!w.valid) { c->set_error("esvo_events_selected_dev: no event window was selected on this context"); return ESVO_ERR_STATE; }
+  if (w.n > *n) { *n = w.n; return ESVO_ERR_CAPACITY; }
+  if (w.n && (!x_dev || !y_dev || !t_dev)) return ESVO_ERR_INVALID_ARG;
+  if (w.n) {
+    ESVO_CUDA_TRY(c, cudaMemcpyAsync(x_dev, w.kx, w.n * 2, cudaMemcpyDeviceToDevice, c->stream));
+    ESVO_CUDA_TRY(c, cudaMemcpyAsync(y_dev, w.ky, w.n * 2, cudaMemcpyDeviceToDevice, c->stream));
+    ESVO_CUDA_TRY(c, cudaMemcpyAsync(t_dev, w.kt, w.n * 8, cudaMemcpyDeviceToDevice, c->stream));
+  }
+  ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+  *n = w.n;
+  return ESVO_OK;
+}
+ESVO_API int esvo_mapping_at_time_selected_dev(esvo_ctx* c, const int64_t* pt, const double* poses, size_t np, uint64_t* counters) {
+  CHECK_CTX(c);
+  if (np && (!pt || !poses)) return ESVO_ERR_INVALID_ARG;
+  if (c->depth > 1) { c->set_error("esvo_mapping_at_time_selected_dev: not available at pipeline depth > 1"); return ESVO_ERR_STATE; }
+  const Ctx::EventWindow& w = c->evw;
+  if (!w.valid) { c->set_error("esvo_mapping_at_time_selected_dev: no event window was selected on this context"); return ESVO_ERR_STATE; }
+  if (!c->obs_set) return ESVO_ERR_STATE;
+  int rc = map_alloc_inputs(c, w.n, np);
+  if (rc) return rc;
+  if ((rc = stage_inputs_packed(c, nullptr, nullptr, nullptr, 0, pt, poses, np))) return rc;   // the poses only
+  c->n_ev = w.n; c->d_ex = w.kx; c->d_ey = w.ky; c->d_et = w.kt;                                // the events in place
+  if ((rc = esvo_run_mapping(c))) return rc;
+  uint64_t ctr[8];
+  if ((rc = fetch_mapping_counters(c, ctr))) return rc;
+  if (counters) std::memcpy(counters, ctr, sizeof(ctr));
+  return ESVO_OK;
+}
+ESVO_API int esvo_init_from_disparity_selected_dev(esvo_ctx* c, const int16_t* disp16, const double T[16], size_t min_points, size_t* n_points,
+                                                   int* accepted) {
+  CHECK_CTX(c);
+  if (!disp16 || !T) return ESVO_ERR_INVALID_ARG;
+  if (c->depth > 1) { c->set_error("esvo_init_from_disparity_selected_dev: not available at pipeline depth > 1"); return ESVO_ERR_STATE; }
+  const Ctx::EventWindow& w = c->evw;
+  if (!w.valid) { c->set_error("esvo_init_from_disparity_selected_dev: no event window was selected on this context"); return ESVO_ERR_STATE; }
+  return init_from_disparity(c, disp16, nullptr, nullptr, w.kx, w.ky, w.n, T, min_points, n_points, accepted);
 }
 
 ESVO_API int esvo_window_download(esvo_ctx* c, int index, esvo_depth_point* out, size_t* n) {

@@ -424,6 +424,9 @@ static int ts_make_room(Ctx* c, int cam, size_t n_new) {
   const size_t drop = s.log_n - keep;
   const int B = 256;
   unsigned g = (unsigned)((drop + B - 1) / B);
+  // scalars[12..13] (one int64): stamp of the first event ever pushed, which the first fold is about to drop.  With the newest
+  // folded stamp it bounds every folded stamp (events.cu answers some lower bounds into the folded part from the two).
+  if (s.log_base == 0) ESVO_CUDA_TRY(c, cudaMemcpyAsync(s.scalars + 12, s.et, 8, cudaMemcpyDeviceToDevice, c->stream));
   ts_scatter_kernel<<<g, B, 0, c->stream>>>(s.ex, s.ey, s.et, drop, s.log_base, c->dc.W, c->dc.H, (long long*)s.base_idx,
                                             s.scalars + 8, (long long*)(s.max_t));
   // scalars[10..11] (one int64): stamp of the newest folded event.  A build at T <= that stamp cannot be answered any more

@@ -421,6 +421,46 @@ ESVO_API int esvo_track_adopt_map_dev(esvo_ctx* ctx, int64_t stamp_ns, size_t* n
  * BATCH_SIZE points; ESVO_ERR_STATE before an adoption. */
 ESVO_API int esvo_track_reset_dev(esvo_ctx* ctx, const double T_world_ref[16], const double T_world_cur_prior[16],
                                   const uint8_t* ts_left);
+/* Event windows read from the time-surface log: the left events the closed loop's mapper and tracker search were pushed into
+ * camera cam's log (esvo_ts_push_events), so the nodes' own event buffers are not needed.  A node's buffer is the logical
+ * buffer [front, total) of global push indices: total = events pushed since esvo_create / esvo_ts_reset, front = where the
+ * node's deque would begin (the mapper caps it at 3e6 events: max(0, total - 3e6); the tracker at 5e6 and clears it on
+ * reset(): max(push index at its last reset, total - 5e6)).  The results equal the host forms on that deque bit for bit.
+ * Refusals, with the reason in esvo_last_error: ESVO_ERR_UNSUPPORTED when the answer depends on events folded out of the
+ * resident log (the newest 1 Mi at least stay resident; see esvo_ts_build), when the camera takes unordered input or its
+ * events were not pushed in time order (the log is in arrival order, the deques are sorted); ESVO_ERR_STATE at pipeline
+ * depth > 1; ESVO_ERR_INVALID_ARG for front outside [0, total].
+ *
+ * replaces: the newest-first walk of esvo_Mapping::dataTransferring (esvo_Mapping.cpp:538-552 SGM, :554-575 BM; host form
+ * frontend::selectSGMEvents / selectCloseEvents) and, with denoise != 0, createDenoisingMask + extractDenoisedEvents
+ * (:282-296,1046-1072).  The walk starts at lower_bound(t_end_ns) and stops before lower_bound(t_begin_ns) (tools::
+ * EventBuffer_lower_bound, utils.h:50-55: toSec() doubles) after at most `budget` events (PROCESS_EVENT_NUM for BM,
+ * PROCESS_EVENT_NUM + 1 for SGM); when no event is at or after t_end_ns, the one-past-the-end slot is skipped but keeps its
+ * place in the budget.  t_begin_ns is the caller's fromSec(max(0, toSec(t_end) - window)), t_begin_ns <= t_end_ns.  With
+ * denoise, the walked events with x < W, y < H draw a 0/255 event map, a 3x3 median (borders replicated) keeps a pixel when at
+ * least 5 of its 9 neighbours are on, and the walked events whose mask value at the flat index y * W + x is 255 are kept in walk
+ * order; without, every walked event is.  At most max_keep are kept.  Deviation: a flat index >= H * W reads outside the
+ * reference's mask (undefined behaviour); such an event is not kept.  The selection stays on the device for the _selected_dev
+ * calls below; *n (may be NULL): its size.  Work and memory are linear in min(budget, resident events): a walk over the whole
+ * resident log (4 Mi events) is allowed, the closed loop's windows are ~1 000 events.  Synchronises once, for the scalars. */
+ESVO_API int esvo_events_window_dev(esvo_ctx* ctx, int cam, int64_t front, int64_t t_begin_ns, int64_t t_end_ns, size_t budget,
+                                    int denoise, size_t max_keep, size_t* n);
+/* replaces: the two EventBuffer_lower_bound calls of esvo_Tracking::curDataTransferring (esvo_Tracking.cpp:240-263), whose
+ * difference + 1 is numEventsSinceLastObs_.  idx_out[i]: lower_bound(t_ns[i]) over [front, total) as a global push index;
+ * k <= 64 stamps per call.  Synchronous.  When some bounds lie among events folded out of the resident log, the others are
+ * still written, those are -1, and the call returns ESVO_ERR_UNSUPPORTED; on every other refusal idx_out is left untouched. */
+ESVO_API int esvo_events_lower_bound_dev(esvo_ctx* ctx, int cam, int64_t front, const int64_t* t_ns, size_t k, int64_t* idx_out);
+/* Read-back of the last selection into device buffers of *n (in: capacity, out: count) events, newest first; synchronous.
+ * ESVO_ERR_STATE without a selection, ESVO_ERR_CAPACITY (with *n set) if it does not fit. */
+ESVO_API int esvo_events_selected_dev(esvo_ctx* ctx, uint16_t* x_dev, uint16_t* y_dev, int64_t* t_ns_dev, size_t* n);
+/* replaces: esvo_Mapping::MappingAtTime (esvo_Mapping.cpp:261-399) on the last selection: esvo_mapping_at_time with the selected
+ * events, used in place.  Poses and counters as there. */
+ESVO_API int esvo_mapping_at_time_selected_dev(esvo_ctx* ctx, const int64_t* pose_t_ns, const double* poses, size_t n_poses,
+                                               uint64_t* counters_out);
+/* replaces: InitializationAtTime downstream of the SGM (esvo_Mapping.cpp:433-492) on the last selection: esvo_init_from_disparity
+ * with the selected events. */
+ESVO_API int esvo_init_from_disparity_selected_dev(esvo_ctx* ctx, const int16_t* disp16, const double T_world_left[16],
+                                                   size_t min_points, size_t* n_points, int* accepted);
 /* Per-stage device timing with CUDA events on the ctx stream.  Stages: 0 time surface, 1 block
  * matching, 2 seed ordering, 3 depth LM, 4 point ordering/culling, 5 fusion+clean+regularise,
  * 6 tracking.  esvo_profile(ctx, stage_mask): bit s switches the timing of stage s on (0 = off, 0xff = all).

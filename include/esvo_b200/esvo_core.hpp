@@ -124,13 +124,18 @@ class TimeSurface {
   bool eventsCallback(const std::vector<esvo::Event>& events) {
     x_.resize(events.size()); y_.resize(events.size()); t_.resize(events.size()); p_.resize(events.size());
     for (size_t i = 0; i < events.size(); ++i) { x_[i] = events[i].x; y_[i] = events[i].y; t_[i] = events[i].ts; p_[i] = events[i].polarity; }
-    return esvo_ts_push_events(cs_->ctx(), cam_, x_.data(), y_.data(), t_.data(), p_.data(), events.size()) == ESVO_OK;
+    if (esvo_ts_push_events(cs_->ctx(), cam_, x_.data(), y_.data(), t_.data(), p_.data(), events.size()) != ESVO_OK) return false;
+    pushed_ += events.size();
+    return true;
   }
+  // events pushed since construction / clearEventQueue: the `total` of the event windows read from this camera's log
+  // (esvo_events_window_dev, esvo_events_lower_bound_dev)
+  size_t eventsPushed() const { return pushed_; }
   // syncCallback -> createTimeSurfaceAtTime (TimeSurface.cpp:52-152,293-311); time_surface_out: H*W mono8 or nullptr
   bool createTimeSurfaceAtTime(int64_t external_sync_time_ns, uint8_t* time_surface_out) {
     return esvo_ts_build(cs_->ctx(), cam_, external_sync_time_ns, nullptr, time_surface_out) == ESVO_OK;
   }
-  void clearEventQueue() { esvo_ts_reset(cs_->ctx(), cam_); }
+  void clearEventQueue() { esvo_ts_reset(cs_->ctx(), cam_); pushed_ = 0; }
   // The reference tolerates stamps that arrive out of order (its insertion sort then re-queues events_.back(),
   // TimeSurface.cpp:410-422).  Off by default here (drivers deliver ordered packets; saves two kernels per push);
   // switch it on for sources that do not guarantee ordering -- results are then identical to the reference's.
@@ -141,6 +146,7 @@ class TimeSurface {
   std::vector<uint16_t> x_, y_;
   std::vector<int64_t> t_;
   std::vector<uint8_t> p_;
+  size_t pushed_ = 0;
 };
 }  // namespace esvo_time_surface
 
@@ -656,12 +662,8 @@ class esvo_Mapping {
   // the reference's parameters, esvo_Mapping.cpp:101-108) -- no OpenCV needed on the node side.
   bool InitializationAtTime(const esvo::StampedTimeSurfaceObs& TS_obs, const std::vector<esvo::Event*>& vEventsPtr_left_SGM,
                             size_t INIT_SGM_DP_NUM_Threshold, size_t* n_points = nullptr) {
-    const int num_disparities = 16 * 3, block_size = 11;                       // esvo_Mapping.cpp:101-105
-    std::vector<int16_t> disp((size_t)cs_->width_ * cs_->height_);
-    if (TS_obs.second.stored_ && !setObservation(TS_obs)) return false;      // a stored pair: the SGM reads the observation
-    if (esvo_sgbm_compute(cs_->ctx(), TS_obs.second.left, TS_obs.second.right, num_disparities, block_size, 8 * block_size * block_size,
-                          32 * block_size * block_size, -1, 0, 11, disp.data()) != ESVO_OK)
-      return false;
+    std::vector<int16_t> disp;
+    if (!disparity(TS_obs, disp)) return false;
     return InitializationAtTime(TS_obs, disp.data(), vEventsPtr_left_SGM, INIT_SGM_DP_NUM_Threshold, n_points);
   }
   void reset() { esvo_mapping_reset(cs_->ctx()); }
@@ -685,9 +687,14 @@ class esvo_Mapping {
       while (i >= 0 && EQ[(size_t)i].ts > e.ts) { EQ[(size_t)i + 1] = EQ[(size_t)i]; --i; }
       EQ[(size_t)(i + 1)] = e;
     }
-    static constexpr size_t MAX_EVENT_QUEUE_LENGTH = 3000000;
     if (EQ.size() > MAX_EVENT_QUEUE_LENGTH) EQ.erase(EQ.begin(), EQ.begin() + (long)(EQ.size() - MAX_EVENT_QUEUE_LENGTH));
   }
+  static constexpr size_t MAX_EVENT_QUEUE_LENGTH = 3000000;
+  // Device form: the left events are in camera 0's time-surface log on this context, total_left of them since it was reset
+  // (esvo_time_surface::TimeSurface::eventsPushed).  events_left_ stays empty; dataTransferring then selects its window and the
+  // denoised subset on the device (esvo_events_window_dev over the deque's place in the log, [max(0, total - 3e6), total)),
+  // and InitializationAtTime / MappingAtTime run on that selection.  events_right_ is never read by the mapper.
+  void eventsCallback(size_t total_left) { log_total_ = total_left; events_in_log_ = true; }
   // timeSurfaceCallback (:716-762): the stereo pair is copied into a history of TS_HISTORY_LENGTH_ entries
   void timeSurfaceCallback(int64_t stamp_ns, const uint8_t* time_surface_left, const uint8_t* time_surface_right) {
     const size_t n = (size_t)cs_->width_ * cs_->height_;
@@ -729,11 +736,18 @@ class esvo_Mapping {
       ++it_end;
     }
     if (!has_obs_) return false;
-    if (ESVO_System_Status_ == "INITIALIZATION")           // SGM (:537-552)
-      frontend::selectSGMEvents(events_left_, TS_obs_.first, BM_half_slice_thickness_, PROCESS_EVENT_NUM_, vEventsPtr_left_SGM_);
+    sel_on_device_ = false;
+    if (ESVO_System_Status_ == "INITIALIZATION") {         // SGM (:537-552)
+      if (events_in_log_) { if (!selectOnDevice(2 * BM_half_slice_thickness_, PROCESS_EVENT_NUM_ + 1, false, PROCESS_EVENT_NUM_ + 1)) return false; }
+      else frontend::selectSGMEvents(events_left_, TS_obs_.first, BM_half_slice_thickness_, PROCESS_EVENT_NUM_, vEventsPtr_left_SGM_);
+    }
     if (ESVO_System_Status_ == "WORKING") {                // BM (:554-603)
-      frontend::selectCloseEvents(events_left_, TS_obs_.first, BM_half_slice_thickness_, PROCESS_EVENT_NUM_, vCloseEventsPtr_left_);
-      vALLEventsPtr_left_ = vCloseEventsPtr_left_;         // both are filled by the same walk (:569-574)
+      if (events_in_log_) {                                // the walk and the denoising step (:282-304) in one device call
+        if (!selectOnDevice(10 * BM_half_slice_thickness_, PROCESS_EVENT_NUM_, bDenoising_, PROCESS_EVENT_NUM_)) return false;
+      } else {
+        frontend::selectCloseEvents(events_left_, TS_obs_.first, BM_half_slice_thickness_, PROCESS_EVENT_NUM_, vCloseEventsPtr_left_);
+        vALLEventsPtr_left_ = vCloseEventsPtr_left_;       // both are filled by the same walk (:569-574)
+      }
       st_map_.clear();
       for (int64_t t : frontend::samplePoseStamps(TS_obs_.first, BM_half_slice_thickness_)) {
         esvo::Pose tr;
@@ -755,16 +769,17 @@ class esvo_Mapping {
     res = LoopResult();
     if (ESVO_System_Status_ == "TERMINATE" || TS_history_.size() < 10) return false;
     { auto _ = calls_.time("mapping.dataTransferring"); dataTransferring(); }
-    if (!has_obs_) return false;
+    if (!error_.empty() || !has_obs_) return false;
     if (ESVO_System_Status_ == "INITIALIZATION" || ESVO_System_Status_ == "RESET") {
       res.ran = 1;
       { auto _ = calls_.time("mapping.InitializationAtTime");
-        res.ok = InitializationAtTime(TS_obs_, vEventsPtr_left_SGM_, INIT_SGM_DP_NUM_Threshold_, &res.n_sgm_points); }
+        res.ok = sel_on_device_ ? initializationOnSelection(&res.n_sgm_points)
+                                : InitializationAtTime(TS_obs_, vEventsPtr_left_SGM_, INIT_SGM_DP_NUM_Threshold_, &res.n_sgm_points); }
       if (res.ok) { auto _ = calls_.time("mapping.publishMappingResults"); publishMappingResults(res); }
     }
     if (ESVO_System_Status_ == "WORKING") {
       res.ran = 2;
-      {
+      if (!sel_on_device_) {                                 // the device form denoised in dataTransferring
         auto _ = calls_.time("mapping.denoising");
         vDenoisedEventsPtr_left_.clear();
         if (bDenoising_) {                                   // :282-296
@@ -776,7 +791,8 @@ class esvo_Mapping {
                                           vCloseEventsPtr_left_.begin() + (long)std::min(vCloseEventsPtr_left_.size(), PROCESS_EVENT_NUM_));
         }
       }
-      { auto _ = calls_.time("mapping.MappingAtTime"); res.ok = MappingAtTime(TS_obs_, vDenoisedEventsPtr_left_, st_map_, &res.ctr); }
+      { auto _ = calls_.time("mapping.MappingAtTime");
+        res.ok = sel_on_device_ ? mappingOnSelection(&res.ctr) : MappingAtTime(TS_obs_, vDenoisedEventsPtr_left_, st_map_, &res.ctr); }
       if (res.ok) { auto _ = calls_.time("mapping.publishMappingResults"); publishMappingResults(res); }
     }
     return res.ok;
@@ -797,7 +813,48 @@ class esvo_Mapping {
   std::vector<esvo::Event*> vEventsPtr_left_SGM_, vALLEventsPtr_left_, vCloseEventsPtr_left_, vDenoisedEventsPtr_left_;
   esvo::StampTransformationMap st_map_;
   esvo::CallTimes calls_;   // host time of each call MappingLoopOnce makes
+  std::string error_;       // device form: why the log could not answer a window (MappingLoopOnce then returned false)
  private:
+  // The device form of a dataTransferring window: the walk from lower_bound(t_obs) back to lower_bound(t_begin), t_begin =
+  // fromSec(max(0, toSec(t_obs) - window)) as selectCloseEventsIn / selectSGMEventsIn compute it, at most `budget` events,
+  // then the denoising mask; at most max_keep are kept.  The selection stays on the device.
+  bool selectOnDevice(double window, size_t budget, bool denoise, size_t max_keep) {
+    const int64_t t_begin = frontend::fromSec(std::max(0.0, frontend::toSec(TS_obs_.first) - window));
+    const int64_t front = log_total_ > MAX_EVENT_QUEUE_LENGTH ? (int64_t)(log_total_ - MAX_EVENT_QUEUE_LENGTH) : 0;
+    if (esvo_events_window_dev(cs_->ctx(), 0, front, t_begin, TS_obs_.first, budget, denoise ? 1 : 0, max_keep, &n_selected_) != ESVO_OK) {
+      error_ = std::string("event window: ") + esvo_last_error(cs_->ctx());
+      return false;
+    }
+    sel_on_device_ = true;
+    return true;
+  }
+  // the SGM of InitializationAtTime (:444): cv::StereoSGBM(0, 48, 11, 968, 3872, -1, 0, 11) on the observation
+  // (esvo_Mapping.cpp:101-108), on the device
+  bool disparity(const esvo::StampedTimeSurfaceObs& TS_obs, std::vector<int16_t>& disp) {
+    const int num_disparities = 16 * 3, block_size = 11;                       // esvo_Mapping.cpp:101-105
+    disp.resize((size_t)cs_->width_ * cs_->height_);
+    if (TS_obs.second.stored_ && !setObservation(TS_obs)) return false;      // a stored pair: the SGM reads the observation
+    return esvo_sgbm_compute(cs_->ctx(), TS_obs.second.left, TS_obs.second.right, num_disparities, block_size, 8 * block_size * block_size,
+                             32 * block_size * block_size, -1, 0, 11, disp.data()) == ESVO_OK;
+  }
+  bool initializationOnSelection(size_t* n_points) {
+    std::vector<int16_t> disp;
+    if (!disparity(TS_obs_, disp)) return false;
+    size_t n = 0; int accepted = 0;
+    if (esvo_init_from_disparity_selected_dev(cs_->ctx(), disp.data(), TS_obs_.second.tr_.data(), INIT_SGM_DP_NUM_Threshold_, &n, &accepted) != ESVO_OK)
+      return false;
+    if (n_points) *n_points = n;
+    return accepted != 0;
+  }
+  bool mappingOnSelection(Counters* out) {
+    if (!setObservation(TS_obs_)) return false;
+    std::vector<int64_t> pt; std::vector<double> poses;
+    for (auto& st : st_map_) { pt.push_back(st.first); poses.insert(poses.end(), st.second.begin(), st.second.end()); }
+    uint64_t c[8];
+    if (esvo_mapping_at_time_selected_dev(cs_->ctx(), pt.data(), poses.data(), pt.size(), c) != ESVO_OK) return false;
+    if (out) *out = Counters{c[0], c[1], c[2], c[3], c[4], c[5], c[6], c[7]};
+    return true;
+  }
   // the observation to the device: the stored pair by its stamp, or the host images (nullptr: the last builds)
   bool setObservation(const esvo::StampedTimeSurfaceObs& TS_obs) {
     const auto& obs = TS_obs.second;
@@ -832,6 +889,8 @@ class esvo_Mapping {
   struct TsPair { std::vector<uint8_t> left, right; size_t id; bool stored; };   // stored: the images are in the device history
   esvo::CameraSystem::Ptr cs_;
   std::deque<esvo::Event> events_left_, events_right_;   // EventQueue (esvo_Mapping.h)
+  size_t log_total_ = 0, n_selected_ = 0;                 // device form: left events in the log; size of the selection
+  bool events_in_log_ = false, sel_on_device_ = false;
   std::map<int64_t, TsPair> TS_history_;
   size_t TS_id_ = 0;
   bool has_obs_ = false;
@@ -1273,10 +1332,14 @@ class esvo_Tracking {
       while (i >= 0 && events_left_[(size_t)i].ts > e.ts) { events_left_[(size_t)i + 1] = events_left_[(size_t)i]; --i; }
       events_left_[(size_t)(i + 1)] = e;
     }
-    static constexpr size_t MAX_EVENT_QUEUE_LENGTH = 5000000;
     if (events_left_.size() > MAX_EVENT_QUEUE_LENGTH)
       events_left_.erase(events_left_.begin(), events_left_.begin() + (long)(events_left_.size() - MAX_EVENT_QUEUE_LENGTH));
   }
+  static constexpr size_t MAX_EVENT_QUEUE_LENGTH = 5000000;
+  // Device form: the left events are in camera 0's time-surface log on this context, total_left of them since it was reset
+  // (esvo_time_surface::TimeSurface::eventsPushed).  events_left_ stays empty; curDataTransferring counts on the device
+  // (esvo_events_lower_bound_dev over the deque's place in the log, [max(push index at the last reset(), total - 5e6), total)).
+  void eventsCallback(size_t total_left) { log_total_ = total_left; events_in_log_ = true; }
   // ---- refDataTransferring (:177-211) ----
   bool refDataTransferring() {
     ref_.t_ = refPCMap_.rbegin()->first;
@@ -1295,16 +1358,14 @@ class esvo_Tracking {
   }
   // ---- curDataTransferring (:213-245) ----
   bool curDataTransferring() {
-    const size_t ev_last = lower_bound_ev(cur_.t_);
+    const int64_t t_last = cur_.t_;
     auto TS_it = TS_history_.rbegin();
     if (cur_.t_ == TS_it->first) return false;        // TS_history may not have been updated yet
     cur_.t_ = TS_it->first;
     cur_.ts_left = TS_it->second.left.empty() ? nullptr : TS_it->second.left.data();   // empty: the newest camera-0 build
     if (ESVO_System_Status_ == "INITIALIZATION" && ets_ == IDLE) cur_.tr_ = ref_.tr_;
     if (ESVO_System_Status_ == "WORKING" || (ESVO_System_Status_ == "INITIALIZATION" && ets_ == WORKING)) cur_.tr_ = T_world_cur_;
-    const size_t ev_cur = lower_bound_ev(cur_.t_);
-    cur_.numEventsSinceLastObs_ = ev_cur - ev_last + 1;
-    return true;
+    return numEventsBetween(t_last, cur_.t_, cur_.numEventsSinceLastObs_);
   }
   // ---- one pass of TrackingLoop's body (:84-171).  Returns true when a pose was produced (then also in T_world_cur_). ----
   bool TrackingLoopOnce() {
@@ -1333,7 +1394,7 @@ class esvo_Tracking {
     ets_ = IDLE;
     return false;
   }
-  void reset() { ets_ = IDLE; TS_id_ = 0; TS_history_.clear(); refPCMap_.clear(); events_left_.clear(); }   // (:247-255)
+  void reset() { ets_ = IDLE; TS_id_ = 0; TS_history_.clear(); refPCMap_.clear(); events_left_.clear(); log_reset_ = log_total_; }   // (:247-255)
   // saveTrajectory (:430-462): per tracked frame "<std::to_string(t.toSec())> tx ty tz qx qy qz qw", fixed notation, precision 9
   // after the stamp; q = Eigen::Quaterniond(R) (esvo::quaternionFromRotation).  The translation is written as Eigen's default
   // IOFormat writes twc.transpose(): every column right-aligned to the widest of the three.  false if the file cannot be opened.
@@ -1370,6 +1431,21 @@ class esvo_Tracking {
     while (lo < hi) { size_t mid = (lo + hi) / 2; if (frontend::toSec(events_left_[mid].ts) < ts) lo = mid + 1; else hi = mid; }
     return lo;
   }
+  // numEventsSinceLastObs_ (:240-263): lower_bound(t_cur) - lower_bound(t_last) + 1.  The reference only logs it
+  // (RegProblemSolverLM.cpp:47-51).  In the device form, a bound that lies among events folded out of the resident log cannot be
+  // answered (ESVO_ERR_UNSUPPORTED); the count is then SIZE_MAX ("unknown") and tracking goes on.  Any other failure (a device
+  // error, unordered input, a front past the log) sets error_ and returns false, which stops the pass.
+  bool numEventsBetween(int64_t t_last, int64_t t_cur, size_t& count) {
+    if (!events_in_log_) { count = lower_bound_ev(t_cur) - lower_bound_ev(t_last) + 1; return true; }
+    const size_t lo = log_total_ > MAX_EVENT_QUEUE_LENGTH ? log_total_ - MAX_EVENT_QUEUE_LENGTH : 0;
+    const int64_t front = (int64_t)std::max(log_reset_, lo), q[2] = {t_last, t_cur};
+    int64_t idx[2] = {-2, -2};
+    const int rc = esvo_events_lower_bound_dev(cs_->ctx(), 0, front, q, 2, idx);
+    if (rc == ESVO_OK) { count = (size_t)(idx[1] - idx[0]) + 1; return true; }
+    if (rc == ESVO_ERR_UNSUPPORTED && (idx[0] == -1 || idx[1] == -1)) { count = SIZE_MAX; return true; }   // folded out
+    error_ = std::string("event count: ") + esvo_last_error(cs_->ctx());
+    return false;
+  }
   struct TsEntry { std::vector<uint8_t> left; size_t id; };
   esvo::CameraSystem::Ptr cs_;
   core::RegProblemType rpType_;
@@ -1378,6 +1454,8 @@ class esvo_Tracking {
   std::map<int64_t, RefMap> refPCMap_;
   std::map<int64_t, TsEntry> TS_history_;
   std::deque<esvo::Event> events_left_;
+  size_t log_total_ = 0, log_reset_ = 0;   // device form: left events in the log; how many there were at the last reset()
+  bool events_in_log_ = false;
   PoseProvider getPoseAt_;
 };
 }  // namespace esvo_core

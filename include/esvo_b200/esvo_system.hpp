@@ -4,8 +4,9 @@
 // the /ESVO_SYSTEM_STATUS parameter.  esvo_System owns one CameraSystem (one esvo_ctx), both TimeSurfaces, the mapper,
 // the tracker and the tf pose buffer both nodes look poses up in, and runs the nodes on a fixed schedule of sync ticks
 // t_k = t0 + k * dt (DESIGN.md section 5):
-//   1. every event with stamp < t_k that has not been delivered goes to both time surfaces, the mapper's left / right
-//      buffers and the tracker's left buffer;
+//   1. every event with stamp < t_k that has not been delivered goes to both time surfaces; the mapper and the tracker read
+//      their left events from camera 0's time-surface log (esvo_events_window_dev, esvo_events_lower_bound_dev) and only
+//      learn how many there are -- their host event buffers stay empty;
 //   2. both time surfaces are built at t_k; the pair goes to the mapper's history, the left image to the tracker's -- on the
 //      device: the mapper's history is the context's time-surface history, the tracker reads the newest camera-0 build;
 //   3. esvo_Tracking::TrackingLoopOnce(); a pose it produces goes into the pose buffer at once (publishPose ->
@@ -66,8 +67,9 @@ class esvo_System {
     const auto c0 = clk::now();
     bool ok;
     { auto _ = calls_.time("ts.eventsCallback"); ok = (left.empty() || ts_left_.eventsCallback(left)) && (right.empty() || ts_right_.eventsCallback(right)); }
-    { auto _ = calls_.time("mapping.eventsCallback"); mapper_.eventsCallback(left, true); mapper_.eventsCallback(right, false); }
-    { auto _ = calls_.time("tracking.eventsCallback"); tracker_.eventsCallback(left); }
+    // the mapper and the tracker read their left events from camera 0's log (esvo_events_*_dev): they get the count only
+    { auto _ = calls_.time("mapping.eventsCallback"); mapper_.eventsCallback(ts_left_.eventsPushed()); }
+    { auto _ = calls_.time("tracking.eventsCallback"); tracker_.eventsCallback(ts_left_.eventsPushed()); }
     { auto _ = calls_.time("ts.createTimeSurfaceAtTime");
       ok = ok && ts_left_.createTimeSurfaceAtTime(rec.t, nullptr) && ts_right_.createTimeSurfaceAtTime(rec.t, nullptr); }
     if (!ok) return stop(std::string("time surface: ") + esvo_last_error(cs_->ctx()), rec);
@@ -85,6 +87,7 @@ class esvo_System {
       mapper_.ESVO_System_Status_ = status_;
       esvo_Mapping::LoopResult r;
       { auto _ = calls_.time("mapping.MappingLoopOnce"); mapper_.MappingLoopOnce(r); }
+      if (!mapper_.error_.empty()) return stop("mapping: " + mapper_.error_, rec);
       status_ = mapper_.ESVO_System_Status_;
       MappingRecord m;
       m.tick = k_; m.ran = r.ran; m.ok = r.ok; m.n_sgm_points = r.n_sgm_points; m.ctr = r.ctr;
