@@ -52,8 +52,8 @@ __device__ __forceinline__ long long lower_bound_log(const int64_t* __restrict__
   return f.base + lo;
 }
 
-// One thread: the two bounds, the one-past-the-end rule and the walk's extent (frontend::selectCloseEventsIn /
-// selectSGMEventsIn).  budget: PROCESS_EVENT_NUM for BM, PROCESS_EVENT_NUM + 1 for SGM.
+// One thread: the two bounds, the one-past-the-end rule and the walk's extent (frontend::selectCloseEvents /
+// selectSGMEvents).  budget: PROCESS_EVENT_NUM for BM, PROCESS_EVENT_NUM + 1 for SGM.
 __global__ void ew_bounds_kernel(const int64_t* __restrict__ et, const int32_t* __restrict__ scal, long long log_base, long long log_n,
                                  long long front, double t_begin, double t_end, long long budget, long long* __restrict__ out) {
   if (threadIdx.x || blockIdx.x) return;

@@ -32,6 +32,15 @@ using StampTransformationMap = std::vector<std::pair<int64_t, Pose>>;   // sorte
 using EventMatchPair = esvo_seed;                                       // core::EventMatchPair
 using DepthPoint = esvo_depth_point;                                    // container::DepthPoint
 
+namespace detail {
+// a StampTransformationMap as the ABI takes it: stamps[n] and row-major poses[16 n]
+inline std::pair<std::vector<int64_t>, std::vector<double>> stampsAndPoses(const StampTransformationMap& st_map) {
+  std::pair<std::vector<int64_t>, std::vector<double>> sp;
+  for (auto& st : st_map) { sp.first.push_back(st.first); sp.second.insert(sp.second.end(), st.second.begin(), st.second.end()); }
+  return sp;
+}
+}  // namespace detail
+
 // container::CameraSystem + the parameter yaml of one node: owns the esvo_ctx of one event stream / GPU.
 class CameraSystem {
  public:
@@ -172,8 +181,7 @@ class EventBM {
     if (!pStampedTsObs_ || !pSt_map_) return;
     const auto& obs = pStampedTsObs_->second;
     if (esvo_set_ts_pair(camSysPtr_->ctx(), obs.left, obs.right, obs.tr_.data()) != ESVO_OK) return;
-    std::vector<int64_t> pt; std::vector<double> poses;
-    for (auto& st : *pSt_map_) { pt.push_back(st.first); poses.insert(poses.end(), st.second.begin(), st.second.end()); }
+    const auto [pt, poses] = esvo::detail::stampsAndPoses(*pSt_map_);
     vEMP.resize(ex_.size());
     size_t n = vEMP.size();
     if (esvo_bm_match(camSysPtr_->ctx(), ex_.data(), ey_.data(), et_.data(), ex_.size(), pt.data(), poses.data(), pt.size(),
@@ -382,74 +390,64 @@ inline int64_t fromSec(double t) {   // ros::Time(double): sec = floor(t), nsec 
   sec += nsec / 1000000000LL; nsec %= 1000000000LL;
   return sec * 1000000000LL + nsec;
 }
+// tools::EventBuffer_lower_bound (utils.h:50-55) over a time-ordered, random-access buffer of esvo::Event: the first event
+// whose stamp is not before t_ns.  It compares toSec() DOUBLES, so stamps that share a double are equal.
+template <class Buffer>
+inline size_t lowerBound(const Buffer& events, int64_t t_ns) {
+  const double ts = toSec(t_ns);
+  size_t lo = 0, hi = events.size();
+  while (lo < hi) { size_t mid = (lo + hi) / 2; if (toSec(events[mid].ts) < ts) lo = mid + 1; else hi = mid; }
+  return lo;
+}
+// The start of a window of window_s seconds that ends at t_end (:542,563): ros::Time(max(0, t_end.toSec() - window_s))
+inline int64_t windowBegin(int64_t t_end_ns, double window_s) { return fromSec(std::max(0.0, toSec(t_end_ns) - window_s)); }
+namespace detail {
+// The walk of dataTransferring's windows: from lower_bound(t_end) back to, not including, lower_bound(windowBegin(t_end,
+// window_s)), at most `budget` events, newest first (:547-551,570-574).  When no event is at/after t_end (the observation
+// stamp is newer than the whole buffer -- the common case online) the reference's first push is deque::end()._M_cur, one
+// slot past the newest event (UB: an unconstructed event); it then still walks back over the newest valid events.  We skip
+// only that slot but keep its place in the budget.
+template <class Buffer>
+inline void walkWindow(Buffer& events, int64_t t_end_ns, double window_s, size_t budget, std::vector<esvo::Event*>& out) {
+  out.clear();
+  if (events.empty()) return;
+  size_t ev_end = lowerBound(events, t_end_ns);
+  const size_t ev_begin = lowerBound(events, windowBegin(t_end_ns, window_s));
+  if (ev_end == events.size() && ev_end != ev_begin && budget > 0) { --ev_end; --budget; }
+  while (ev_end != ev_begin && out.size() < budget) { out.push_back(&events[ev_end]); --ev_end; }
+}
+}  // namespace detail
+// events_left: a time-ordered std::vector or std::deque (the node's EventQueue) of esvo::Event
 template <class EventBuffer>
-inline void selectCloseEventsIn(EventBuffer& events_left /* time-ordered */, int64_t t_end_ns, double BM_half_slice_thickness,
-                              size_t PROCESS_EVENT_NUM, std::vector<esvo::Event*>& vCloseEventsPtr_left) {
-  vCloseEventsPtr_left.clear();
-  if (events_left.empty()) return;
-  const double t_end = toSec(t_end_ns);
-  const int64_t t_begin_ns = fromSec(std::max(0.0, t_end - 10 * BM_half_slice_thickness));
-  auto lower = [&](int64_t t) {   // tools::EventBuffer_lower_bound (utils.h:50-55): compares toSec() DOUBLES (stamps that share a double are equal)
-    const double ts = toSec(t);
-    size_t lo = 0, hi = events_left.size();
-    while (lo < hi) { size_t mid = (lo + hi) / 2; if (toSec(events_left[mid].ts) < ts) lo = mid + 1; else hi = mid; }
-    return lo;
-  };
-  size_t ev_end = lower(t_end_ns);
-  const size_t ev_begin = lower(t_begin_ns);
-  // The walk starts AT lower_bound(t_end) and stops before lower_bound(t_begin) (:570-574).  When no event is at/after
-  // t_end (the observation stamp is newer than the whole buffer -- the common case online) the reference's first push is
-  // deque::end()._M_cur, one slot past the newest event (UB: an unconstructed event); it then still walks back over the
-  // newest valid events.  We skip only that slot but keep its place in the PROCESS_EVENT_NUM budget.
-  size_t budget = PROCESS_EVENT_NUM;
-  if (ev_end == events_left.size() && ev_end != ev_begin && budget > 0) { --ev_end; --budget; }
-  while (ev_end != ev_begin && vCloseEventsPtr_left.size() < budget) {
-    vCloseEventsPtr_left.push_back(&events_left[ev_end]);
-    --ev_end;
-  }
+inline void selectCloseEvents(EventBuffer& events_left, int64_t t_end_ns, double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM,
+                              std::vector<esvo::Event*>& vCloseEventsPtr_left) {
+  detail::walkWindow(events_left, t_end_ns, 10 * BM_half_slice_thickness, PROCESS_EVENT_NUM, vCloseEventsPtr_left);
 }
 //  * selectSGMEvents: the INITIALIZATION branch of dataTransferring (:538-552) -- window 2*BM_half_slice_thickness and
 //    `<=` instead of `<` on the count (one event more than PROCESS_EVENT_NUM).
 template <class EventBuffer>
-inline void selectSGMEventsIn(EventBuffer& events_left, int64_t t_end_ns, double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM,
+inline void selectSGMEvents(EventBuffer& events_left, int64_t t_end_ns, double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM,
                             std::vector<esvo::Event*>& vEventsPtr_left_SGM) {
-  vEventsPtr_left_SGM.clear();
-  if (events_left.empty()) return;
-  const int64_t t_begin_ns = fromSec(std::max(0.0, toSec(t_end_ns) - 2 * BM_half_slice_thickness));
-  auto lower = [&](int64_t t) {
-    const double ts = toSec(t);
-    size_t lo = 0, hi = events_left.size();
-    while (lo < hi) { size_t mid = (lo + hi) / 2; if (toSec(events_left[mid].ts) < ts) lo = mid + 1; else hi = mid; }
-    return lo;
-  };
-  size_t ev_end = lower(t_end_ns);
-  const size_t ev_begin = lower(t_begin_ns);
-  size_t budget = PROCESS_EVENT_NUM + 1;      // `<=` on the count: one event more than PROCESS_EVENT_NUM
-  if (ev_end == events_left.size() && ev_end != ev_begin) { --ev_end; --budget; }   // skip the one-past-the-end slot (see selectCloseEvents)
-  while (ev_end != ev_begin && vEventsPtr_left_SGM.size() < budget) { vEventsPtr_left_SGM.push_back(&events_left[ev_end]); --ev_end; }
-}
-inline void selectCloseEvents(std::vector<esvo::Event>& events_left /* time-ordered */, int64_t t_end_ns, double BM_half_slice_thickness,
-                              size_t PROCESS_EVENT_NUM, std::vector<esvo::Event*>& vCloseEventsPtr_left) {
-  selectCloseEventsIn(events_left, t_end_ns, BM_half_slice_thickness, PROCESS_EVENT_NUM, vCloseEventsPtr_left);
-}
-inline void selectCloseEvents(std::deque<esvo::Event>& events_left /* time-ordered: the node's EventQueue */, int64_t t_end_ns,
-                              double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM, std::vector<esvo::Event*>& vCloseEventsPtr_left) {
-  selectCloseEventsIn(events_left, t_end_ns, BM_half_slice_thickness, PROCESS_EVENT_NUM, vCloseEventsPtr_left);
-}
-inline void selectSGMEvents(std::vector<esvo::Event>& events_left, int64_t t_end_ns, double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM,
-                            std::vector<esvo::Event*>& vEventsPtr_left_SGM) {
-  selectSGMEventsIn(events_left, t_end_ns, BM_half_slice_thickness, PROCESS_EVENT_NUM, vEventsPtr_left_SGM);
-}
-inline void selectSGMEvents(std::deque<esvo::Event>& events_left, int64_t t_end_ns, double BM_half_slice_thickness, size_t PROCESS_EVENT_NUM,
-                            std::vector<esvo::Event*>& vEventsPtr_left_SGM) {
-  selectSGMEventsIn(events_left, t_end_ns, BM_half_slice_thickness, PROCESS_EVENT_NUM, vEventsPtr_left_SGM);
+  detail::walkWindow(events_left, t_end_ns, 2 * BM_half_slice_thickness, PROCESS_EVENT_NUM + 1, vEventsPtr_left_SGM);
 }
 inline std::vector<int64_t> samplePoseStamps(int64_t t_end_ns, double BM_half_slice_thickness) {
   std::vector<int64_t> out;
   const double t_end = toSec(t_end_ns);
-  int64_t t_tmp = fromSec(std::max(0.0, t_end - 10 * BM_half_slice_thickness));
+  int64_t t_tmp = windowBegin(t_end_ns, 10 * BM_half_slice_thickness);
   while (toSec(t_tmp) <= t_end) { out.push_back(t_tmp); t_tmp = fromSec(toSec(t_tmp) + 0.05 * BM_half_slice_thickness); }
   return out;
+}
+//  * queueEvents: eventsCallback's EventQueue (esvo_Mapping.cpp:669-703, esvo_Tracking.cpp:294-321, esvo_MVStereo.cpp:
+//    746-790): each event is insertion-sorted in behind the queued ones with a stamp not above its own, then the oldest
+//    events above max_length are dropped.
+inline void queueEvents(std::deque<esvo::Event>& EQ, const std::vector<esvo::Event>& events, size_t max_length) {
+  for (const esvo::Event& e : events) {
+    EQ.push_back(e);
+    long i = (long)EQ.size() - 2;
+    while (i >= 0 && EQ[(size_t)i].ts > e.ts) { EQ[(size_t)i + 1] = EQ[(size_t)i]; --i; }
+    EQ[(size_t)(i + 1)] = e;
+  }
+  if (EQ.size() > max_length) EQ.erase(EQ.begin(), EQ.begin() + (long)(EQ.size() - max_length));
 }
 //  * createDenoisingMask / extractDenoisedEvents (esvo_Mapping.cpp:1046-1072, bDenoising_): binary event map of ALL
 //    window events -> cv::medianBlur 3x3 (on a 0/255 image: a pixel survives iff at least 5 of its 3x3 neighbours,
@@ -476,6 +474,19 @@ inline void extractDenoisedEvents(const std::vector<esvo::Event*>& vCloseEventsP
   for (esvo::Event* e : vCloseEventsPtr) {
     if (vEdgeEventsPtr.size() >= maxNum) break;
     if (mask[(size_t)e->y * col + e->x] == 255) vEdgeEventsPtr.push_back(e);
+  }
+}
+//  * denoise: the denoising step of MappingAtTime (esvo_Mapping.cpp:282-304, esvo_MVStereo.cpp:385-405): with bDenoising the
+//    mask of all window events keeps at most maxNum of the close events, without it the first maxNum of them are kept.
+inline void denoise(const std::vector<esvo::Event*>& vAllEventsPtr, const std::vector<esvo::Event*>& vCloseEventsPtr, bool bDenoising,
+                    size_t row, size_t col, size_t maxNum, std::vector<esvo::Event*>& vDenoisedEventsPtr) {
+  vDenoisedEventsPtr.clear();
+  if (bDenoising) {
+    std::vector<uint8_t> mask;
+    createDenoisingMask(vAllEventsPtr, mask, row, col);
+    extractDenoisedEvents(vCloseEventsPtr, vDenoisedEventsPtr, mask, col, maxNum);
+  } else {
+    vDenoisedEventsPtr.assign(vCloseEventsPtr.begin(), vCloseEventsPtr.begin() + (long)std::min(vCloseEventsPtr.size(), maxNum));
   }
 }
 //  * the local-map hand-off of publishPointCloud (esvo_Mapping.cpp:909-953): p_world = R p_cam + t as pcl::PointXYZ
@@ -533,17 +544,24 @@ template <class EventBuffer>
 inline bool selectEMEvents(EventBuffer& events, int64_t t_low_ns, int64_t t_up_ns, size_t EM_numEventMatching,
                            std::vector<esvo::Event*>& vEventsPtr) {
   vEventsPtr.clear();
-  auto lower = [&](int64_t t) {   // tools::EventBuffer_lower_bound (utils.h:50-55): toSec() doubles
-    const double ts = toSec(t);
-    size_t lo = 0, hi = events.size();
-    while (lo < hi) { size_t mid = (lo + hi) / 2; if (toSec(events[mid].ts) < ts) lo = mid + 1; else hi = mid; }
-    return lo;
-  };
-  size_t lo = lower(t_low_ns);
-  const size_t up = lower(t_up_ns);
+  size_t lo = lowerBound(events, t_low_ns);
+  const size_t up = lowerBound(events, t_up_ns);
   if (up <= lo + 1) return false;
   while (lo != up - 1 && vEventsPtr.size() <= EM_numEventMatching) vEventsPtr.push_back(&events[lo++]);
   return true;
+}
+//  * findObservation: the observation of dataTransferring (esvo_Mapping.cpp:501-534, esvo_MVStereo.cpp:560-576) -- the
+//    newest history entry but one, walking back to the oldest, the first one poseAt gives a pose for (then in tr).  Returns
+//    history.end() when there is none.  The history holds at least two entries.
+template <class Entry, class PoseAt>
+inline typename std::map<int64_t, Entry>::const_iterator findObservation(const std::map<int64_t, Entry>& history, PoseAt&& poseAt,
+                                                                         esvo::Pose& tr) {
+  auto it = std::next(history.rbegin());                 // in case the tf is behind the most current TS
+  for (;; ++it) {
+    tr = esvo::Pose{};
+    if (poseAt(it->first, tr)) return std::prev(it.base());
+    if (it->first == history.begin()->first) return history.end();
+  }
 }
 }  // namespace frontend
 }  // namespace esvo_core
@@ -632,15 +650,7 @@ class esvo_Mapping {
   struct Counters { uint64_t n_events, n_seeds, n_solved, n_culled, n_fusions, bm_evals, lm_evals, map_size; };
   bool MappingAtTime(const esvo::StampedTimeSurfaceObs& TS_obs, const std::vector<esvo::Event*>& vCloseEventsPtr_left,
                      const esvo::StampTransformationMap& st_map, Counters* out = nullptr) {
-    if (!setObservation(TS_obs)) return false;
-    std::vector<uint16_t> ex, ey; std::vector<int64_t> et, pt; std::vector<double> poses;
-    for (auto* e : vCloseEventsPtr_left) { ex.push_back(e->x); ey.push_back(e->y); et.push_back(e->ts); }
-    for (auto& st : st_map) { pt.push_back(st.first); poses.insert(poses.end(), st.second.begin(), st.second.end()); }
-    uint64_t c[8];
-    if (esvo_mapping_at_time(cs_->ctx(), ex.data(), ey.data(), et.data(), ex.size(), pt.data(), poses.data(), pt.size(), c) != ESVO_OK)
-      return false;
-    if (out) *out = Counters{c[0], c[1], c[2], c[3], c[4], c[5], c[6], c[7]};
-    return true;
+    return mapping(TS_obs, &vCloseEventsPtr_left, st_map, out);
   }
   // InitializationAtTime (esvo_Mapping.cpp:433-492).  The SGM stays where it is -- the node's
   //   sgbm_->compute(TS_left, TS_right, dispMap)       (cv::StereoSGBM(0,48,11,968,3872,-1,0,11), esvo_Mapping.cpp:101-108,444)
@@ -680,14 +690,7 @@ class esvo_Mapping {
   std::string ESVO_System_Status_ = "INITIALIZATION";
   // eventsCallback (:669-703) for events_left_ / events_right_: insertion-sorted, capped at 3e6
   void eventsCallback(const std::vector<esvo::Event>& events, bool left) {
-    std::deque<esvo::Event>& EQ = left ? events_left_ : events_right_;
-    for (const esvo::Event& e : events) {
-      EQ.push_back(e);
-      long i = (long)EQ.size() - 2;
-      while (i >= 0 && EQ[(size_t)i].ts > e.ts) { EQ[(size_t)i + 1] = EQ[(size_t)i]; --i; }
-      EQ[(size_t)(i + 1)] = e;
-    }
-    if (EQ.size() > MAX_EVENT_QUEUE_LENGTH) EQ.erase(EQ.begin(), EQ.begin() + (long)(EQ.size() - MAX_EVENT_QUEUE_LENGTH));
+    frontend::queueEvents(left ? events_left_ : events_right_, events, MAX_EVENT_QUEUE_LENGTH);
   }
   static constexpr size_t MAX_EVENT_QUEUE_LENGTH = 3000000;
   // Device form: the left events are in camera 0's time-surface log on this context, total_left of them since it was reset
@@ -715,27 +718,21 @@ class esvo_Mapping {
   bool dataTransferring() {
     TS_obs_ = esvo::StampedTimeSurfaceObs(); has_obs_ = false;
     if (TS_history_.size() <= 10) return false;
-    auto it_end = TS_history_.rbegin();
-    ++it_end;                                             // in case the tf is behind the most current TS
-    const int64_t t_oldest = TS_history_.begin()->first;
-    while (!has_obs_) {
-      esvo::Pose tr{};
-      if (ESVO_System_Status_ == "INITIALIZATION") { tr = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}; has_obs_ = true; }
-      if (ESVO_System_Status_ == "WORKING") {
-        if (getPoseAt_ && getPoseAt_(it_end->first, tr)) has_obs_ = true;
-        else if (ESVO_System_Status_ != "WORKING") return false;
-      }
-      if (has_obs_) {
-        TS_obs_.first = it_end->first;
-        TS_obs_.second.stored_ = it_end->second.stored;
-        TS_obs_.second.left = it_end->second.stored ? nullptr : it_end->second.left.data();
-        TS_obs_.second.right = it_end->second.stored ? nullptr : it_end->second.right.data();
-        TS_obs_.second.id_ = it_end->second.id; TS_obs_.second.setTransformation(tr);
-      }
-      if (it_end->first == t_oldest) break;
-      ++it_end;
-    }
-    if (!has_obs_) return false;
+    bool lost = false;   // a failed look-up took the status off WORKING: the walk stops there and dataTransferring fails (:521-527)
+    esvo::Pose tr;
+    const auto it = frontend::findObservation(TS_history_, [&](int64_t t, esvo::Pose& T) {
+      if (ESVO_System_Status_ == "INITIALIZATION") { T = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}; return true; }
+      if (ESVO_System_Status_ != "WORKING") return false;
+      if (getPoseAt_ && getPoseAt_(t, T)) return true;
+      return lost = ESVO_System_Status_ != "WORKING";
+    }, tr);
+    if (lost || it == TS_history_.end()) return false;
+    TS_obs_.first = it->first;
+    TS_obs_.second.stored_ = it->second.stored;
+    TS_obs_.second.left = it->second.stored ? nullptr : it->second.left.data();
+    TS_obs_.second.right = it->second.stored ? nullptr : it->second.right.data();
+    TS_obs_.second.id_ = it->second.id; TS_obs_.second.setTransformation(tr);
+    has_obs_ = true;
     sel_on_device_ = false;
     if (ESVO_System_Status_ == "INITIALIZATION") {         // SGM (:537-552)
       if (events_in_log_) { if (!selectOnDevice(2 * BM_half_slice_thickness_, PROCESS_EVENT_NUM_ + 1, false, PROCESS_EVENT_NUM_ + 1)) return false; }
@@ -781,18 +778,11 @@ class esvo_Mapping {
       res.ran = 2;
       if (!sel_on_device_) {                                 // the device form denoised in dataTransferring
         auto _ = calls_.time("mapping.denoising");
-        vDenoisedEventsPtr_left_.clear();
-        if (bDenoising_) {                                   // :282-296
-          std::vector<uint8_t> mask;
-          frontend::createDenoisingMask(vALLEventsPtr_left_, mask, (size_t)cs_->height_, (size_t)cs_->width_);
-          frontend::extractDenoisedEvents(vCloseEventsPtr_left_, vDenoisedEventsPtr_left_, mask, (size_t)cs_->width_, PROCESS_EVENT_NUM_);
-        } else {                                             // :297-304
-          vDenoisedEventsPtr_left_.assign(vCloseEventsPtr_left_.begin(),
-                                          vCloseEventsPtr_left_.begin() + (long)std::min(vCloseEventsPtr_left_.size(), PROCESS_EVENT_NUM_));
-        }
+        frontend::denoise(vALLEventsPtr_left_, vCloseEventsPtr_left_, bDenoising_, (size_t)cs_->height_, (size_t)cs_->width_, PROCESS_EVENT_NUM_,
+                          vDenoisedEventsPtr_left_);
       }
       { auto _ = calls_.time("mapping.MappingAtTime");
-        res.ok = sel_on_device_ ? mappingOnSelection(&res.ctr) : MappingAtTime(TS_obs_, vDenoisedEventsPtr_left_, st_map_, &res.ctr); }
+        res.ok = mapping(TS_obs_, sel_on_device_ ? nullptr : &vDenoisedEventsPtr_left_, st_map_, &res.ctr); }
       if (res.ok) { auto _ = calls_.time("mapping.publishMappingResults"); publishMappingResults(res); }
     }
     return res.ok;
@@ -815,11 +805,11 @@ class esvo_Mapping {
   esvo::CallTimes calls_;   // host time of each call MappingLoopOnce makes
   std::string error_;       // device form: why the log could not answer a window (MappingLoopOnce then returned false)
  private:
-  // The device form of a dataTransferring window: the walk from lower_bound(t_obs) back to lower_bound(t_begin), t_begin =
-  // fromSec(max(0, toSec(t_obs) - window)) as selectCloseEventsIn / selectSGMEventsIn compute it, at most `budget` events,
-  // then the denoising mask; at most max_keep are kept.  The selection stays on the device.
+  // The device form of a dataTransferring window: the walk of selectCloseEvents / selectSGMEvents from lower_bound(t_obs) back
+  // to lower_bound(frontend::windowBegin(t_obs, window)), at most `budget` events, then the denoising mask; at most max_keep
+  // are kept.  The selection stays on the device.
   bool selectOnDevice(double window, size_t budget, bool denoise, size_t max_keep) {
-    const int64_t t_begin = frontend::fromSec(std::max(0.0, frontend::toSec(TS_obs_.first) - window));
+    const int64_t t_begin = frontend::windowBegin(TS_obs_.first, window);
     const int64_t front = log_total_ > MAX_EVENT_QUEUE_LENGTH ? (int64_t)(log_total_ - MAX_EVENT_QUEUE_LENGTH) : 0;
     if (esvo_events_window_dev(cs_->ctx(), 0, front, t_begin, TS_obs_.first, budget, denoise ? 1 : 0, max_keep, &n_selected_) != ESVO_OK) {
       error_ = std::string("event window: ") + esvo_last_error(cs_->ctx());
@@ -846,12 +836,17 @@ class esvo_Mapping {
     if (n_points) *n_points = n;
     return accepted != 0;
   }
-  bool mappingOnSelection(Counters* out) {
-    if (!setObservation(TS_obs_)) return false;
-    std::vector<int64_t> pt; std::vector<double> poses;
-    for (auto& st : st_map_) { pt.push_back(st.first); poses.insert(poses.end(), st.second.begin(), st.second.end()); }
+  // MappingAtTime on the host events, or with events == nullptr on the device selection of dataTransferring
+  bool mapping(const esvo::StampedTimeSurfaceObs& TS_obs, const std::vector<esvo::Event*>* events, const esvo::StampTransformationMap& st_map,
+               Counters* out) {
+    if (!setObservation(TS_obs)) return false;
+    std::vector<uint16_t> ex, ey; std::vector<int64_t> et;
+    if (events) for (auto* e : *events) { ex.push_back(e->x); ey.push_back(e->y); et.push_back(e->ts); }
+    const auto [pt, poses] = esvo::detail::stampsAndPoses(st_map);
     uint64_t c[8];
-    if (esvo_mapping_at_time_selected_dev(cs_->ctx(), pt.data(), poses.data(), pt.size(), c) != ESVO_OK) return false;
+    const int rc = events ? esvo_mapping_at_time(cs_->ctx(), ex.data(), ey.data(), et.data(), ex.size(), pt.data(), poses.data(), pt.size(), c)
+                          : esvo_mapping_at_time_selected_dev(cs_->ctx(), pt.data(), poses.data(), pt.size(), c);
+    if (rc != ESVO_OK) return false;
     if (out) *out = Counters{c[0], c[1], c[2], c[3], c[4], c[5], c[6], c[7]};
     return true;
   }
@@ -919,16 +914,10 @@ class MVStereoFrontEnd {
   bool eventsCallback(const std::vector<esvo::Event>& events, bool left) {
     if (events.empty()) return false;
     bool was_reset = false;
-    std::deque<esvo::Event>* EQ = left ? &events_left_ : &events_right_;
-    if (!EQ->empty() && inconsistent(events[0].ts, EQ->back().ts)) { reset(); was_reset = true; }
-    for (const esvo::Event& e : events) {
-      EQ->push_back(e);
-      long i = (long)EQ->size() - 2;
-      while (i >= 0 && (*EQ)[(size_t)i].ts > e.ts) { (*EQ)[(size_t)i + 1] = (*EQ)[(size_t)i]; --i; }
-      (*EQ)[(size_t)(i + 1)] = e;
-    }
+    std::deque<esvo::Event>& EQ = left ? events_left_ : events_right_;
+    if (!EQ.empty() && inconsistent(events[0].ts, EQ.back().ts)) { reset(); was_reset = true; }
     static constexpr size_t MAX_EVENT_QUEUE_LENGTH = 3000000;   // clearEventQueue (:782-790)
-    if (EQ->size() > MAX_EVENT_QUEUE_LENGTH) EQ->erase(EQ->begin(), EQ->begin() + (long)(EQ->size() - MAX_EVENT_QUEUE_LENGTH));
+    frontend::queueEvents(EQ, events, MAX_EVENT_QUEUE_LENGTH);
     return was_reset;
   }
   // timeSurfaceCallback (:792-838): dt against the newest stamp in TS_history_; dt < 0 or >= 0.5 s resets.  The pair is
@@ -984,21 +973,13 @@ class MVStereoFrontEnd {
   bool dataTransferring() {
     clearSelection();
     if (TS_history_.size() <= 10) return false;
-    auto it_end = TS_history_.rbegin();
-    ++it_end;                                             // in case the tf is behind the most current TS
-    const int64_t t_oldest = TS_history_.begin()->first;
-    while (!has_obs_) {
-      esvo::Pose tr;
-      if (getPoseAt(it_end->first, tr)) {
-        TS_obs_.first = it_end->first;
-        TS_obs_.second.left = it_end->second.left.data(); TS_obs_.second.right = it_end->second.right.data();
-        TS_obs_.second.id_ = it_end->second.id; TS_obs_.second.setTransformation(tr);
-        has_obs_ = true;
-      }
-      if (it_end->first == t_oldest) break;
-      ++it_end;
-    }
-    if (!has_obs_) return false;
+    esvo::Pose tr;
+    const auto it = frontend::findObservation(TS_history_, [&](int64_t t, esvo::Pose& T) { return getPoseAt(t, T); }, tr);
+    if (it == TS_history_.end()) return false;
+    TS_obs_.first = it->first;
+    TS_obs_.second.left = it->second.left.data(); TS_obs_.second.right = it->second.right.data();
+    TS_obs_.second.id_ = it->second.id; TS_obs_.second.setTransformation(tr);
+    has_obs_ = true;
     if (msm_ == 0 || msm_ == 2) {
       t_lowBound_ = TS_history_.begin()->first; t_upBound_ = TS_history_.rbegin()->first;
       std::vector<esvo::Event*> l, r;
@@ -1022,15 +1003,7 @@ class MVStereoFrontEnd {
   // The BM branch of MappingAtTime before the matcher (:385-405): the denoising mask of all window events keeps at most
   // PROCESS_EVENT_NUM of the close events, or, without denoising, the first PROCESS_EVENT_NUM of them.
   void denoise() {
-    vDenoisedEventsPtr_left_.clear();
-    if (bDenoising_) {
-      std::vector<uint8_t> mask;
-      frontend::createDenoisingMask(vALLEventsPtr_left_, mask, H_, W_);
-      frontend::extractDenoisedEvents(vCloseEventsPtr_left_, vDenoisedEventsPtr_left_, mask, W_, PROCESS_EVENT_NUM_);
-    } else {
-      vDenoisedEventsPtr_left_.assign(vCloseEventsPtr_left_.begin(),
-                                      vCloseEventsPtr_left_.begin() + (long)std::min(vCloseEventsPtr_left_.size(), PROCESS_EVENT_NUM_));
-    }
+    frontend::denoise(vALLEventsPtr_left_, vCloseEventsPtr_left_, bDenoising_, H_, W_, PROCESS_EVENT_NUM_, vDenoisedEventsPtr_left_);
   }
   // The host part of one MappingLoop pass (:196-225): the TS_history_.size() >= 10 gate, dataTransferring, the skip when no
   // observation was loaded (TS_obs_ empty), and in BM modes the denoising.  true: MappingAtTime is due on TS_obs_ -- also
@@ -1325,16 +1298,7 @@ class esvo_Tracking {
     while (TS_history_.size() > TS_HISTORY_LENGTH_) TS_history_.erase(TS_history_.begin());
   }
   // eventsCallback: insertion-sorted event buffer, capped at 5e6 (:294-321)
-  void eventsCallback(const std::vector<esvo::Event>& events) {
-    for (const esvo::Event& e : events) {
-      events_left_.push_back(e);
-      long i = (long)events_left_.size() - 2;
-      while (i >= 0 && events_left_[(size_t)i].ts > e.ts) { events_left_[(size_t)i + 1] = events_left_[(size_t)i]; --i; }
-      events_left_[(size_t)(i + 1)] = e;
-    }
-    if (events_left_.size() > MAX_EVENT_QUEUE_LENGTH)
-      events_left_.erase(events_left_.begin(), events_left_.begin() + (long)(events_left_.size() - MAX_EVENT_QUEUE_LENGTH));
-  }
+  void eventsCallback(const std::vector<esvo::Event>& events) { frontend::queueEvents(events_left_, events, MAX_EVENT_QUEUE_LENGTH); }
   static constexpr size_t MAX_EVENT_QUEUE_LENGTH = 5000000;
   // Device form: the left events are in camera 0's time-surface log on this context, total_left of them since it was reset
   // (esvo_time_surface::TimeSurface::eventsPushed).  events_left_ stays empty; curDataTransferring counts on the device
@@ -1425,18 +1389,12 @@ class esvo_Tracking {
   std::vector<esvo::Pose> lPose_;
   core::RegProblemSolverLM rpSolver_;
  private:
-  size_t lower_bound_ev(int64_t t) const {   // tools::EventBuffer_lower_bound (utils.h:50-55): toSec() doubles
-    const double ts = frontend::toSec(t);
-    size_t lo = 0, hi = events_left_.size();
-    while (lo < hi) { size_t mid = (lo + hi) / 2; if (frontend::toSec(events_left_[mid].ts) < ts) lo = mid + 1; else hi = mid; }
-    return lo;
-  }
   // numEventsSinceLastObs_ (:240-263): lower_bound(t_cur) - lower_bound(t_last) + 1.  The reference only logs it
   // (RegProblemSolverLM.cpp:47-51).  In the device form, a bound that lies among events folded out of the resident log cannot be
   // answered (ESVO_ERR_UNSUPPORTED); the count is then SIZE_MAX ("unknown") and tracking goes on.  Any other failure (a device
   // error, unordered input, a front past the log) sets error_ and returns false, which stops the pass.
   bool numEventsBetween(int64_t t_last, int64_t t_cur, size_t& count) {
-    if (!events_in_log_) { count = lower_bound_ev(t_cur) - lower_bound_ev(t_last) + 1; return true; }
+    if (!events_in_log_) { count = frontend::lowerBound(events_left_, t_cur) - frontend::lowerBound(events_left_, t_last) + 1; return true; }
     const size_t lo = log_total_ > MAX_EVENT_QUEUE_LENGTH ? log_total_ - MAX_EVENT_QUEUE_LENGTH : 0;
     const int64_t front = (int64_t)std::max(log_reset_, lo), q[2] = {t_last, t_cur};
     int64_t idx[2] = {-2, -2};

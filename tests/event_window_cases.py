@@ -2,8 +2,8 @@
 esvo_events_lower_bound_dev), and their host forms in numpy.
 
 A case is a left event stream pushed into camera 0 in batches, and queries against it:
-  * ("window", front, t_begin_ns, t_end_ns, budget, denoise, max_keep) -- the walk of frontend::selectCloseEventsIn /
-    selectSGMEventsIn over the deque events[front:total], then createDenoisingMask + extractDenoisedEvents;
+  * ("window", front, t_begin_ns, t_end_ns, budget, denoise, max_keep) -- the walk of frontend::selectCloseEvents /
+    selectSGMEvents over the deque events[front:total], then createDenoisingMask + extractDenoisedEvents;
   * ("lower_bound", front, stamps) -- tools::EventBuffer_lower_bound over the same deque, as global push indices.
 Streams are built deterministically.  expect() gives the host form's answer, or None where the resident log of the product
 cannot answer (log model: LOG_CAP events, the oldest folded out when a push would overflow, keeping LOG_CAP / 4)."""
@@ -39,7 +39,7 @@ def t_begin_for(t_end_ns, window_s):
 
 
 def walk(secs, t_begin_ns, t_end_ns, budget):
-    """selectCloseEventsIn / selectSGMEventsIn on a deque whose toSec() stamps are secs: indices into the deque, newest first."""
+    """selectCloseEvents / selectSGMEvents on a deque whose toSec() stamps are secs: indices into the deque, newest first."""
     v_end, v_begin = to_sec([t_end_ns, t_begin_ns])
     ev_end = int(np.searchsorted(secs, v_end, side="left"))
     ev_begin = int(np.searchsorted(secs, v_begin, side="left"))

@@ -1,5 +1,5 @@
 """Event windows read from the time-surface log (include/esvo_b200.h: esvo_events_window_dev, esvo_events_lower_bound_dev and the
-_selected_dev frames) against their host forms byte for byte: the walk of frontend::selectCloseEventsIn / selectSGMEventsIn
+_selected_dev frames) against their host forms byte for byte: the walk of frontend::selectCloseEvents / selectSGMEvents
 (tests/indep_numpy.py) over the node's deque, createDenoisingMask + extractDenoisedEvents (cv2.medianBlur), and
 tools::EventBuffer_lower_bound; refusals where the resident log cannot answer; the mapping frames on a selection against the
 host-array calls on the same events; and the closed loop with Denoising off against its restatement."""
