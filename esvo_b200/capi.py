@@ -81,6 +81,17 @@ DEPTH_POINT_DTYPE = np.dtype([
     ("p_cam", "<f8", (3,)), ("T_world_cam", "<f8", (16,))], align=True)
 assert SEED_DTYPE.itemsize == 8 * (2 + 2 + 2 + 1 + 16 + 3)
 assert DEPTH_POINT_DTYPE.itemsize == 8 + 8 * (2 + 5 + 1 + 3 + 16)
+# dvs_msgs/Event as serialised in a ROS bag (esvo_ts_push_event_array): packed, little-endian, 13 bytes
+EVENT_WIRE_DTYPE = np.dtype([("x", "<u2"), ("y", "<u2"), ("sec", "<u4"), ("nsec", "<u4"), ("polarity", "u1")])
+assert EVENT_WIRE_DTYPE.itemsize == 13
+
+
+def pack_events(x, y, t_ns, pol):
+    """SoA events -> wire records (stamp split as ros::Time: sec = t // 1e9, nsec = t % 1e9); pol bytes are kept as given."""
+    t = np.asarray(t_ns, np.int64)
+    r = np.empty(t.size, EVENT_WIRE_DTYPE)
+    r["x"] = x; r["y"] = y; r["sec"] = t // 1_000_000_000; r["nsec"] = t % 1_000_000_000; r["polarity"] = pol
+    return r
 
 
 class EsvoError(RuntimeError):
@@ -243,6 +254,21 @@ class Backend:
 
     def ts_reset(self, cam):
         self._call("ts_reset", [C.c_int], cam)
+
+    def ts_push_event_array(self, cam, runs, ok=(0,)):
+        """esvo_ts_push_event_array: runs is a list of byte buffers (bytes, bytearray, uint8 arrays), each a whole number of
+        13-byte dvs_msgs/Event wire records (EVENT_WIRE_DTYPE).  Returns the return code (in ok, else EsvoError)."""
+        bufs = [np.frombuffer(r, np.uint8) if not isinstance(r, np.ndarray) else _arr(r, np.uint8).ravel() for r in runs]
+        for b in bufs:
+            assert b.size % EVENT_WIRE_DTYPE.itemsize == 0
+        ptrs = (C.c_void_p * max(1, len(bufs)))(*[b.ctypes.data if b.size else None for b in bufs])
+        ns = (C.c_size_t * max(1, len(bufs)))(*[b.size // EVENT_WIRE_DTYPE.itemsize for b in bufs])
+        return self._call("ts_push_event_array", [C.c_int, C.c_void_p, C.c_void_p, C.c_int], cam, C.cast(ptrs, C.c_void_p),
+                          C.cast(ns, C.c_void_p), len(bufs), ok=ok)
+
+    def ts_push_event_array_dev(self, cam, packed_dev_ptr, n, ok=(0,)):
+        """esvo_ts_push_event_array_dev: n wire records at the device address packed_dev_ptr (an int, any alignment)."""
+        return self._call("ts_push_event_array_dev", [C.c_int, C.c_void_p, C.c_size_t], cam, C.c_void_p(packed_dev_ptr), n, ok=ok)
 
     # ---- mapping ----
     def set_ts_pair(self, ts_left, ts_right, T_world_left):

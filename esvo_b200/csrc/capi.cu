@@ -455,6 +455,19 @@ ESVO_API int esvo_ts_push_events(esvo_ctx* c, int cam, const uint16_t* x, const 
   ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->s_tsc[cam]));
   return ESVO_OK;
 }
+ESVO_API int esvo_ts_push_event_array(esvo_ctx* c, int cam, const uint8_t* const* runs, const size_t* n_events, int n_runs) {
+  CHECK_CTX(c);
+  if (cam < 0 || cam > 1 || n_runs < 0 || (n_runs && (!runs || !n_events))) return ESVO_ERR_INVALID_ARG;
+  for (int k = 0; k < n_runs; ++k) if (n_events[k] && !runs[k]) return ESVO_ERR_INVALID_ARG;
+  StreamScope sc(c, c->s_tsc[cam]);
+  return ts_push_packed_host(c, cam, runs, n_events, n_runs);
+}
+ESVO_API int esvo_ts_push_event_array_dev(esvo_ctx* c, int cam, const uint8_t* packed_dev, size_t n) {
+  CHECK_CTX(c);
+  if (cam < 0 || cam > 1 || (n && !packed_dev)) return ESVO_ERR_INVALID_ARG;
+  StreamScope sc(c, c->s_tsc[cam]);
+  return ts_push_packed(c, cam, packed_dev, n, nullptr);
+}
 ESVO_API int esvo_run_ts_build(esvo_ctx* c, int cam, int64_t T) {
   CHECK_CTX(c);
   if (cam < 0 || cam > 1) return ESVO_ERR_INVALID_ARG;

@@ -49,6 +49,58 @@ __global__ void ts_ingest_kernel(const uint16_t* __restrict__ sx, const uint16_t
   if (x >= W || y >= H) return;
   atomicMax(&idx_grid[(size_t)y * W + x], gbase + (long long)i);
 }
+// ---- packed source: dvs_msgs/Event wire records, as a ROS bag's EventArray messages carry them.  Record i is 13 bytes at
+// src + 13 i, little-endian and unaligned: u16 x | u16 y | u32 sec | u32 nsec | u8 polarity.  Each warp stages the bytes of
+// its 32 records, and of the record before them (the order test), through shared memory with aligned 4-byte loads; only
+// the words at the two ends of the whole input are read byte by byte.  Then each lane decodes its record from shared memory.
+// RAW = false: same writes, order flag and scatter as ts_ingest_kernel.  RAW = true: decode into the unordered path's
+// raw_* staging only (its run-max kernels do the rest).
+constexpr int kPackRec = 13, kPackWords = (kPackRec * 33 + 3 + 3) / 4;   // 32 records + the one before, any alignment
+__device__ __forceinline__ long long packed_stamp(const uint8_t* r) {   // ros::Time::toNSec(): sec * 1e9 + nsec, 64-bit
+  const unsigned sec = r[4] | (r[5] << 8) | (r[6] << 16) | ((unsigned)r[7] << 24);
+  const unsigned nsec = r[8] | (r[9] << 8) | (r[10] << 16) | ((unsigned)r[11] << 24);
+  return (long long)sec * 1000000000LL + (long long)nsec;
+}
+template <bool RAW>
+__global__ void __launch_bounds__(256) ts_ingest_packed_kernel(const uint8_t* __restrict__ src, size_t n,
+                                                               uint16_t* __restrict__ ex, uint16_t* __restrict__ ey,
+                                                               int64_t* __restrict__ et, uint8_t* __restrict__ ep, long long gbase,
+                                                               int W, int H, long long* __restrict__ idx_grid,
+                                                               int32_t* __restrict__ scalars, const long long* __restrict__ max_t) {
+  __shared__ uint32_t stage[8][kPackWords];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const size_t i0 = (blockIdx.x * (size_t)blockDim.x) + (size_t)w * 32;   // first record of this warp
+  if (i0 >= n) return;
+  const size_t i = i0 + lane;
+  const uintptr_t lo = (uintptr_t)src, hi = lo + n * kPackRec;           // the input's bytes [lo, hi)
+  const uintptr_t b0 = lo + (i0 > 0 ? i0 - 1 : 0) * kPackRec;            // the previous record's first byte (or the first one)
+  const uintptr_t b1 = lo + min(n, i0 + 32) * kPackRec;
+  const uintptr_t a0 = b0 & ~(uintptr_t)3;
+  const int nw = (int)((b1 - a0 + 3) >> 2);
+  for (int k = lane; k < nw; k += 32) {
+    const uintptr_t a = a0 + 4 * (uintptr_t)k;
+    uint32_t v;
+    if (a >= lo && a + 4 <= hi) v = *(const uint32_t*)a;
+    else {   // an end word of the input: only its bytes inside [lo, hi)
+      v = 0;
+      for (int q = 0; q < 4; ++q) if (a + q >= lo && a + q < hi) v |= (uint32_t)*(const uint8_t*)(a + q) << (8 * q);
+    }
+    stage[w][k] = v;
+  }
+  __syncwarp();
+  if (i >= n) return;
+  const uint8_t* sb = (const uint8_t*)stage[w];
+  const uint8_t* r = sb + (lo + i * kPackRec - a0);
+  const int x = r[0] | (r[1] << 8), y = r[2] | (r[3] << 8);
+  const long long t = packed_stamp(r);
+  const uint8_t pol = r[12] != 0;   // the ROS bool
+  ex[i] = (uint16_t)x; ey[i] = (uint16_t)y; et[i] = t; ep[i] = pol;
+  if (RAW) return;
+  if (i > 0 && packed_stamp(r - kPackRec) > t) scalars[1] = 1;
+  if (i == 0 && *max_t > t) scalars[1] = 1;
+  if (x >= W || y >= H) return;
+  atomicMax(&idx_grid[(size_t)y * W + x], gbase + (long long)i);
+}
 // second pass: the winner of each pixel caches its stamp and polarity
 __global__ void ts_scatter_fix_kernel(const uint16_t* __restrict__ ex, const uint16_t* __restrict__ ey,
                                       const int64_t* __restrict__ et, const uint8_t* __restrict__ ep, size_t n,
@@ -410,6 +462,8 @@ void ts_free(Ctx* c, int cam) {
                 s.tmp_t, s.tmp_pol, s.cnt, s.out_idx, s.img_med, s.img_out, s.map1, s.map2, s.scalars, s.max_t,
                 s.fwd_lut, s.fwd_head, s.fwd_next, s.fwd_val, s.raw_x, s.raw_y, s.raw_t, s.raw_p, s.raw_eff, s.agg, s.back, s.pack_dev};
   for (void* p : ps) if (p) cudaFree(p);
+  if (s.h_pack) cudaFreeHost(s.h_pack);
+  if (s.ev_pack) cudaEventDestroy(s.ev_pack);
   s = TsState();
 }
 
@@ -457,6 +511,38 @@ static const uint8_t* packet_span(const uint16_t* x, const uint16_t* y, const in
   return span <= n * 13 + 64 ? lo : nullptr;
 }
 
+// Unordered input (esvo_ts_set_unordered_input): the raw batch staging, block aggregates and carried event, grown to n.
+static int ts_raw_reserve(Ctx* c, TsState& s, size_t n) {
+  const int nb = (int)((n + 1023) / 1024);
+  if (!s.back) { ESVO_CUDA_TRY(c, dmalloc(&s.back, 10)); ESVO_CUDA_TRY(c, cudaMemsetAsync(s.back, 0, 80, c->stream)); }
+  if (n > s.raw_cap) {
+    ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    void* olds[] = {s.raw_x, s.raw_y, s.raw_t, s.raw_p, s.raw_eff};
+    for (void* q : olds) if (q) cudaFree(q);
+    s.raw_cap = std::max<size_t>(n, 1 << 16);
+    ESVO_CUDA_TRY(c, dmalloc(&s.raw_x, s.raw_cap)); ESVO_CUDA_TRY(c, dmalloc(&s.raw_y, s.raw_cap)); ESVO_CUDA_TRY(c, dmalloc(&s.raw_t, s.raw_cap));
+    ESVO_CUDA_TRY(c, dmalloc(&s.raw_p, s.raw_cap)); ESVO_CUDA_TRY(c, dmalloc(&s.raw_eff, s.raw_cap));
+  }
+  if ((size_t)nb * 4 > s.agg_cap) {
+    ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    if (s.agg) cudaFree(s.agg);
+    s.agg_cap = std::max<size_t>((size_t)nb * 4, 1024);
+    ESVO_CUDA_TRY(c, dmalloc(&s.agg, s.agg_cap));
+  }
+  return ESVO_OK;
+}
+// Unordered input: the running arg-max of the stamps picks each arrival's effective event, which goes to the log at off.
+static void ts_runmax_push(Ctx* c, TsState& s, const uint16_t* sx, const uint16_t* sy, const int64_t* st, const uint8_t* sp, size_t n,
+                           size_t off, long long gbase) {
+  const int nb = (int)((n + 1023) / 1024), B = 256;
+  const unsigned g = (unsigned)((n + B - 1) / B);
+  ts_runmax_block_kernel<<<nb, 1024, 0, c->stream>>>(st, (int)n, s.raw_eff, (long long*)s.agg, nb);
+  ts_runmax_carry_kernel<<<1, 32, 0, c->stream>>>((long long*)s.agg, nb, sx, sy, st, sp, (long long*)s.back);
+  ts_effective_kernel<<<g, B, 0, c->stream>>>(sx, sy, st, sp, (int)n, s.raw_eff, (const long long*)s.agg, nb, (const long long*)s.back,
+                                              s.ex + off, s.ey + off, s.et + off, s.ep + off, gbase, c->dc.W, c->dc.H, (long long*)s.cur_idx);
+  c->launches += 3;
+}
+
 int ts_push(Ctx* c, int cam, const uint16_t* x, const uint16_t* y, const int64_t* t, const uint8_t* p, size_t n, bool dev_src) {
   if (n == 0) return ESVO_OK;
   size_t span = 0;
@@ -471,22 +557,7 @@ int ts_push(Ctx* c, int cam, const uint16_t* x, const uint16_t* y, const int64_t
   if (dev_src || s.unordered) s.host_knows = false;
   else if (s.host_knows) { if (t[n - 1] >= s.host_max_t) s.host_max_t = t[n - 1]; else s.host_knows = false; }
   if (s.unordered) {
-    const int nb = (int)((n + 1023) / 1024);
-    if (!s.back) { ESVO_CUDA_TRY(c, dmalloc(&s.back, 10)); ESVO_CUDA_TRY(c, cudaMemsetAsync(s.back, 0, 80, c->stream)); }
-    if (n > s.raw_cap) {
-      ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-      void* olds[] = {s.raw_x, s.raw_y, s.raw_t, s.raw_p, s.raw_eff};
-      for (void* q : olds) if (q) cudaFree(q);
-      s.raw_cap = std::max<size_t>(n, 1 << 16);
-      ESVO_CUDA_TRY(c, dmalloc(&s.raw_x, s.raw_cap)); ESVO_CUDA_TRY(c, dmalloc(&s.raw_y, s.raw_cap)); ESVO_CUDA_TRY(c, dmalloc(&s.raw_t, s.raw_cap));
-      ESVO_CUDA_TRY(c, dmalloc(&s.raw_p, s.raw_cap)); ESVO_CUDA_TRY(c, dmalloc(&s.raw_eff, s.raw_cap));
-    }
-    if ((size_t)nb * 4 > s.agg_cap) {
-      ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-      if (s.agg) cudaFree(s.agg);
-      s.agg_cap = std::max<size_t>((size_t)nb * 4, 1024);
-      ESVO_CUDA_TRY(c, dmalloc(&s.agg, s.agg_cap));
-    }
+    if ((rc = ts_raw_reserve(c, s, n))) return rc;
     const uint16_t *sx = x, *sy = y; const int64_t* st = t; const uint8_t* sp = p;
     if (!dev_src) {
       ESVO_CUDA_TRY(c, cudaMemcpyAsync(s.raw_x, x, n * 2, cudaMemcpyHostToDevice, c->stream));
@@ -495,11 +566,7 @@ int ts_push(Ctx* c, int cam, const uint16_t* x, const uint16_t* y, const int64_t
       if (p) ESVO_CUDA_TRY(c, cudaMemcpyAsync(s.raw_p, p, n, cudaMemcpyHostToDevice, c->stream));
       sx = s.raw_x; sy = s.raw_y; st = s.raw_t; sp = p ? s.raw_p : nullptr;
     }
-    ts_runmax_block_kernel<<<nb, 1024, 0, c->stream>>>(st, (int)n, s.raw_eff, (long long*)s.agg, nb);
-    ts_runmax_carry_kernel<<<1, 32, 0, c->stream>>>((long long*)s.agg, nb, sx, sy, st, sp, (long long*)s.back);
-    ts_effective_kernel<<<g, B, 0, c->stream>>>(sx, sy, st, sp, (int)n, s.raw_eff, (const long long*)s.agg, nb, (const long long*)s.back,
-                                                s.ex + off, s.ey + off, s.et + off, s.ep + off, gbase, c->dc.W, c->dc.H, (long long*)s.cur_idx);
-    c->launches += 3;
+    ts_runmax_push(c, s, sx, sy, st, sp, n, off, gbase);
   } else if (dev_src) {
     ts_ingest_kernel<<<g, B, 0, c->stream>>>(x, y, t, p, n, s.ex + off, s.ey + off, s.et + off, s.ep + off, gbase, c->dc.W, c->dc.H,
                                              (long long*)s.cur_idx, s.scalars, (const long long*)s.max_t);
@@ -534,6 +601,79 @@ int ts_push(Ctx* c, int cam, const uint16_t* x, const uint16_t* y, const int64_t
   c->prof_end(pe);
   s.log_n += n;
   return ESVO_OK;
+}
+
+// n dvs_msgs/Event wire records (13 bytes each, any alignment) in device memory.  Everything after the decode is ts_push's:
+// the same log, push indices, order flag, fold and refusals.  host_last_t: the stamp of the last record when the host knows
+// it (the host form below), else null -- as for ts_push's host and device sources.
+int ts_push_packed(Ctx* c, int cam, const uint8_t* src, size_t n, const int64_t* host_last_t) {
+  if (n == 0) return ESVO_OK;
+  TsState& s = c->ts[cam];
+  int rc = ts_make_room(c, cam, n);
+  if (rc) return rc;
+  const size_t off = s.log_n;
+  cudaEvent_t pe = c->prof_begin(0);
+  const int B = 256;
+  const unsigned g = (unsigned)((n + B - 1) / B);
+  const long long gbase = s.log_base + (long long)off;
+  if (!host_last_t || s.unordered) s.host_knows = false;
+  else if (s.host_knows) { if (*host_last_t >= s.host_max_t) s.host_max_t = *host_last_t; else s.host_knows = false; }
+  if (s.unordered) {
+    if ((rc = ts_raw_reserve(c, s, n))) return rc;
+    ts_ingest_packed_kernel<true><<<g, B, 0, c->stream>>>(src, n, s.raw_x, s.raw_y, s.raw_t, s.raw_p, gbase, c->dc.W, c->dc.H, nullptr,
+                                                          nullptr, nullptr);
+    c->launches += 1;
+    ts_runmax_push(c, s, s.raw_x, s.raw_y, s.raw_t, s.raw_p, n, off, gbase);
+  } else {
+    ts_ingest_packed_kernel<false><<<g, B, 0, c->stream>>>(src, n, s.ex + off, s.ey + off, s.et + off, s.ep + off, gbase, c->dc.W,
+                                                           c->dc.H, (long long*)s.cur_idx, s.scalars, (const long long*)s.max_t);
+  }
+  ts_scatter_fix_kernel<<<g, B, 0, c->stream>>>(s.ex + off, s.ey + off, s.et + off, s.ep + off, n, gbase, c->dc.W, c->dc.H,
+                                                (const long long*)s.cur_idx, (long long*)s.cur_t, s.cur_pol, (long long*)s.max_t);
+  c->launches += 2;
+  c->prof_end(pe);
+  s.log_n += n;
+  return ESVO_OK;
+}
+
+// Host runs of wire records (e.g. the event blocks of several EventArray messages in a memory-mapped bag): gathered with
+// memcpy into this camera's pinned staging block, one H2D copy, then ts_push_packed on the copy.  The staging block is
+// reused once the previous copy out of it has completed, so the caller's runs are free again on return.
+int ts_push_packed_host(Ctx* c, int cam, const uint8_t* const* runs, const size_t* n_events, int n_runs) {
+  TsState& s = c->ts[cam];
+  size_t n = 0;
+  for (int k = 0; k < n_runs; ++k) n += n_events[k];
+  if (n == 0) return ESVO_OK;
+  if (n > s.log_cap / 2) { c->set_error("event batch larger than half the resident log"); return ESVO_ERR_CAPACITY; }
+  const size_t bytes = n * kPackRec;
+  if (s.ev_pack) ESVO_CUDA_TRY(c, cudaEventSynchronize(s.ev_pack));
+  else ESVO_CUDA_TRY(c, cudaEventCreateWithFlags(&s.ev_pack, cudaEventDisableTiming));
+  if (bytes > s.h_pack_cap) {
+    if (s.h_pack) cudaFreeHost(s.h_pack);
+    s.h_pack = nullptr;
+    s.h_pack_cap = std::max<size_t>(2 * bytes, (size_t)1 << 20);
+    ESVO_CUDA_TRY(c, cudaMallocHost((void**)&s.h_pack, s.h_pack_cap));
+  }
+  if (bytes > s.pack_cap) {
+    ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
+    if (s.pack_dev) cudaFree(s.pack_dev);
+    s.pack_dev = nullptr;
+    s.pack_cap = std::max<size_t>(2 * bytes, (size_t)1 << 20);
+    ESVO_CUDA_TRY(c, dmalloc(&s.pack_dev, s.pack_cap));
+  }
+  uint8_t* d = s.h_pack;
+  for (int k = 0; k < n_runs; ++k) {
+    if (!n_events[k]) continue;
+    std::memcpy(d, runs[k], n_events[k] * kPackRec);
+    d += n_events[k] * kPackRec;
+  }
+  const uint8_t* last = d - kPackRec;
+  uint32_t sec, nsec;
+  std::memcpy(&sec, last + 4, 4); std::memcpy(&nsec, last + 8, 4);
+  const int64_t t_last = (int64_t)sec * 1000000000LL + (int64_t)nsec;
+  ESVO_CUDA_TRY(c, cudaMemcpyAsync(s.pack_dev, s.h_pack, bytes, cudaMemcpyHostToDevice, c->stream));
+  ESVO_CUDA_TRY(c, cudaEventRecord(s.ev_pack, c->stream));
+  return ts_push_packed(c, cam, s.pack_dev, n, &t_last);
 }
 
 int ts_run_build(Ctx* c, int cam, int64_t T) {

@@ -19,9 +19,9 @@
 #include <fstream>
 
 #include "esvo_b200/esvo_system.hpp"
+#include "system_common.hpp"
 
 template <class T> static bool rd(std::ifstream& f, T* p, size_t n) { f.read((char*)p, (std::streamsize)(n * sizeof(T))); return (bool)f; }
-template <class T> static void wr(std::ofstream& o, const T* p, size_t n) { o.write((const char*)p, (std::streamsize)(n * sizeof(T))); }
 
 int main(int argc, char** argv) {
   if (argc < 4) { std::printf("usage: system_loop <scenario.bin> <result.bin> <trajectory.txt> [calls.txt]\n"); return 64; }
@@ -31,7 +31,7 @@ int main(int argc, char** argv) {
   if (!rd(f, &W, 1) || !rd(f, &H, 1) || !rd(f, &rig, 1) || !rd(f, &t0, 1) || !rd(f, &dt, 1) || !rd(f, &n_ticks, 1) ||
       !rd(f, &mapping_every, 1) || !rd(f, &profile, 1) || !rd(f, &n_ovr, 1) || rig != 0)
     return 65;
-  // calib/hkust + cfg/{mapping,tracking}/*_hkust.yaml (the values esvo_b200/configs.py uses)
+  // calib/hkust (the values esvo_b200/configs.py uses); parameters: cfg/{mapping,tracking}/*_hkust.yaml (system_common.hpp)
   esvo_calib l{}, r{};
   l.width = r.width = W; l.height = r.height = H;
   const double Kl[9] = {263.796, 0, 176.994, 0, 263.738, 124.373, 0, 0, 1}, Dl[4] = {-0.386589, 0.157241, 0.000322143, 6.13759e-06};
@@ -43,16 +43,7 @@ int main(int argc, char** argv) {
   double Pr[12]; std::memcpy(Pr, Pl, sizeof(Pl)); Pr[3] = -13.8634;
   std::memcpy(l.K, Kl, 72); std::memcpy(l.D, Dl, 32); std::memcpy(l.R, Rl, 72); std::memcpy(l.P, Pl, 96);
   std::memcpy(r.K, Kr, 72); std::memcpy(r.D, Dr, 32); std::memcpy(r.R, Rr, 72); std::memcpy(r.P, Pr, 96);
-  esvo_params p; esvo_default_params(&p);
-  p.decay_ms = 30.0; p.ignore_polarity = 1; p.median_blur_kernel_size = 1; p.max_event_queue_len = 20; p.time_surface_mode = 0;
-  p.patch_size_x = 15; p.patch_size_y = 7; p.bm_step = 1; p.bm_zncc_threshold = 0.1; p.bm_updown = 0; p.lsnorm = ESVO_LSNORM_TDIST; p.max_iteration = 10;
-  p.age_vis_threshold = 1; p.fusion_strategy = ESVO_FUSION_CONST_FRAMES; p.num_thread_mapping = 4;
-  p.trk_patch_size_x = p.trk_patch_size_y = 1; p.trk_kernel_size = 5; p.trk_lsnorm = ESVO_TRK_LSNORM_HUBER; p.trk_huber_threshold = 50;
-  p.trk_max_registration_points = 2000; p.trk_max_iteration = 10; p.trk_min_num_events = 1000; p.trk_batch_size = 500;
-  p.invdepth_min_range = 0.25; p.invdepth_max_range = 2.0; p.residual_vis_threshold = 20; p.stdvar_vis_threshold = 0.15;
-  p.fusion_radius = 0; p.max_num_fusion_frames = 20; p.max_num_fusion_points = 4000; p.smooth_time_surface = 0; p.regularization = 1;
-  p.reg_radius = 5; p.reg_min_neighbours = 8; p.reg_min_close_neighbours = 8; p.td_nu = 2.1897; p.td_scale = 16.6397;
-  p.bm_min_disparity = 1; p.bm_max_disparity = 40;
+  esvo_params p = esvo_examples::hkustParams();
   esvo_core::esvo_System::Config cfg;
   cfg.t0_ns = t0; cfg.dt_ns = dt; cfg.mapping_every = mapping_every;
   for (int i = 0; i < n_ovr; ++i) {
@@ -92,37 +83,5 @@ int main(int argc, char** argv) {
   }
   esvo_sync(cs->ctx());
   const double wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - w0).count();
-  double prof_ms[8] = {0}; uint64_t prof_n[8] = {0};
-  if (profile) esvo_profile_read(cs->ctx(), prof_ms, prof_n);
-  std::vector<esvo::DepthPoint> map;
-  sys.getMap(map);
-  if (!sys.saveTrajectory(argv[3])) { std::printf("cannot write %s\n", argv[3]); return 66; }
-
-  std::ofstream o(argv[2], std::ios::binary);
-  const int32_t hdr[4] = {(int32_t)sys.ticks_.size(), (int32_t)sys.mapping_.size(), (int32_t)map.size(), sys.error_.empty() ? 0 : 1};
-  wr(o, hdr, 4);
-  for (const auto& tk : sys.ticks_) {
-    const int32_t st[2] = {tk.status == "INITIALIZATION" ? 0 : tk.status == "WORKING" ? 1 : 2, tk.has_pose ? 1 : 0};
-    const double tm[3] = {tk.ts_ms, tk.tracking_ms, tk.mapping_ms};
-    wr(o, &tk.t, 1); wr(o, st, 2); wr(o, tk.T.data(), 16); wr(o, tm, 3);
-  }
-  for (const auto& m : sys.mapping_) {
-    const int32_t a[4] = {(int32_t)m.tick, m.ran, m.ok ? 1 : 0, m.published ? 1 : 0};
-    const uint64_t b[10] = {m.n_sgm_points, m.ctr.n_events, m.ctr.n_seeds, m.ctr.n_solved, m.ctr.n_culled, m.ctr.n_fusions,
-                            m.ctr.bm_evals, m.ctr.lm_evals, m.ctr.map_size, m.cloud_points};
-    wr(o, a, 4); wr(o, b, 10); wr(o, &m.stamp, 1);
-  }
-  wr(o, map.data(), map.size());
-  wr(o, &wall_ms, 1); wr(o, prof_ms, 8); wr(o, prof_n, 8);
-  if (argc > 4) {
-    std::FILE* cf = std::fopen(argv[4], "w");
-    if (!cf) { std::printf("cannot write %s\n", argv[4]); return 66; }
-    for (const auto& e : sys.callTimes().ms) std::fprintf(cf, "%s %.6f %zu\n", e.first.c_str(), e.second.first, e.second.second);
-    std::fclose(cf);
-  }
-  size_t n_pose = 0;
-  for (const auto& tk : sys.ticks_) n_pose += tk.has_pose ? 1 : 0;
-  std::printf("system loop: %zu ticks, %zu poses, status %s, map %zu, %.1f ms%s%s\n", sys.ticks_.size(), n_pose, sys.status_.c_str(), map.size(), wall_ms,
-              sys.error_.empty() ? "" : ", stopped: ", sys.error_.c_str());
-  return 0;
+  return esvo_examples::writeOutputs(sys, *cs, profile != 0, wall_ms, argv[2], argv[3], argc > 4 ? argv[4] : nullptr);
 }

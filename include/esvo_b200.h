@@ -194,6 +194,7 @@ ESVO_API int esvo_ts_push_events(esvo_ctx* ctx, int cam, const uint16_t* x, cons
  * pushes it returns ESVO_ERR_UNSUPPORTED and changes nothing. */
 ESVO_API int esvo_ts_set_unordered_input(esvo_ctx* ctx, int cam, int enable);
 
+
 /* replaces: TimeSurface::createTimeSurfaceAtTime (TimeSurface.cpp:52-152) incl.
  * EventQueueMat::getMostRecentEventBeforeT (TimeSurface.h:52-75).
  * idx_grid_out (H*W, may be NULL): index, in push order since create/reset, of the event each
@@ -482,4 +483,6 @@ ESVO_API const char* esvo_version(void);
 #ifdef __cplusplus
 }
 #endif
+
+#include "esvo_b200_bag.h"   /* the packed event ingest (no oracle counterpart) */
 #endif /* ESVO_B200_H_ */

@@ -27,6 +27,8 @@
 namespace esvo {
 
 struct Event { uint16_t x, y; int64_t ts; bool polarity; };            // dvs_msgs::Event
+// n dvs_msgs::Event wire records (13 bytes each, as serialised in a ROS bag) at data; see esvo_ts_push_event_array
+struct EventRun { const uint8_t* data = nullptr; size_t n = 0; };
 using Pose = std::array<double, 16>;                                    // Transformation (T_world_cam, row-major)
 using StampTransformationMap = std::vector<std::pair<int64_t, Pose>>;   // sorted by stamp
 using EventMatchPair = esvo_seed;                                       // core::EventMatchPair
@@ -137,6 +139,16 @@ class TimeSurface {
     pushed_ += events.size();
     return true;
   }
+  // The same on packed runs of wire records (the events of one or more EventArray messages): copied as they are and
+  // decoded on the device (esvo_ts_push_event_array), no per-event host work.
+  bool eventsCallback(const std::vector<esvo::EventRun>& runs) {
+    run_ptr_.clear(); run_n_.clear();
+    size_t n = 0;
+    for (const auto& r : runs) { run_ptr_.push_back(r.data); run_n_.push_back(r.n); n += r.n; }
+    if (esvo_ts_push_event_array(cs_->ctx(), cam_, run_ptr_.data(), run_n_.data(), (int)runs.size()) != ESVO_OK) return false;
+    pushed_ += n;
+    return true;
+  }
   // events pushed since construction / clearEventQueue: the `total` of the event windows read from this camera's log
   // (esvo_events_window_dev, esvo_events_lower_bound_dev)
   size_t eventsPushed() const { return pushed_; }
@@ -155,6 +167,8 @@ class TimeSurface {
   std::vector<uint16_t> x_, y_;
   std::vector<int64_t> t_;
   std::vector<uint8_t> p_;
+  std::vector<const uint8_t*> run_ptr_;
+  std::vector<size_t> run_n_;
   size_t pushed_ = 0;
 };
 }  // namespace esvo_time_surface

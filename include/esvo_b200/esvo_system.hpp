@@ -59,6 +59,34 @@ class esvo_System {
   int64_t nextTick() const { return cfg_.t0_ns + (int64_t)k_ * cfg_.dt_ns; }
   // One sync tick.  left / right: the events with stamp < nextTick() not delivered yet, time-ordered.  false once stopped.
   bool SpinOnce(const std::vector<esvo::Event>& left, const std::vector<esvo::Event>& right) {
+    return spin([&] { return (left.empty() || ts_left_.eventsCallback(left)) && (right.empty() || ts_right_.eventsCallback(right)); });
+  }
+  // The same tick with the events as packed runs of wire records (e.g. EventArray messages of a ROS bag,
+  // esvo::RosBagEvents::takeBefore): same schedule, records and outputs as the vector form on the same events.
+  bool SpinOnce(const std::vector<esvo::EventRun>& left, const std::vector<esvo::EventRun>& right) {
+    return spin([&] { return ts_left_.eventsCallback(left) && ts_right_.eventsCallback(right); });
+  }
+  // the fused map the mapper holds (DepthMap element order)
+  void getMap(std::vector<esvo::DepthPoint>& out) { core::DepthFusion f(cs_); f.getElements(out); }
+  bool saveTrajectory(const std::string& path) const { return tracker_.saveTrajectory(path); }
+  // host time of each call SpinOnce makes, and of each call MappingLoopOnce makes (names "mapping.*" inside it)
+  esvo::CallTimes callTimes() const {
+    esvo::CallTimes all = calls_;
+    for (const auto& e : mapper_.calls_.ms) all.ms[e.first] = e.second;
+    return all;
+  }
+
+  const Config& config() const { return cfg_; }
+  std::string status_ = "INITIALIZATION";   // /ESVO_SYSTEM_STATUS
+  std::string error_;
+  std::vector<TickRecord> ticks_;
+  std::vector<MappingRecord> mapping_;
+  esvo::PoseBuffer poses_;
+
+ private:
+  // one sync tick; push() hands the tick's events to both time surfaces
+  template <class Push>
+  bool spin(Push&& push) {
     if (status_ == "TERMINATE") return false;
     using clk = std::chrono::steady_clock;
     auto ms = [](clk::time_point a, clk::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
@@ -66,7 +94,7 @@ class esvo_System {
     rec.t = nextTick();
     const auto c0 = clk::now();
     bool ok;
-    { auto _ = calls_.time("ts.eventsCallback"); ok = (left.empty() || ts_left_.eventsCallback(left)) && (right.empty() || ts_right_.eventsCallback(right)); }
+    { auto _ = calls_.time("ts.eventsCallback"); ok = push(); }
     // the mapper and the tracker read their left events from camera 0's log (esvo_events_*_dev): they get the count only
     { auto _ = calls_.time("mapping.eventsCallback"); mapper_.eventsCallback(ts_left_.eventsPushed()); }
     { auto _ = calls_.time("tracking.eventsCallback"); tracker_.eventsCallback(ts_left_.eventsPushed()); }
@@ -102,24 +130,6 @@ class esvo_System {
     ++k_;
     return true;
   }
-  // the fused map the mapper holds (DepthMap element order)
-  void getMap(std::vector<esvo::DepthPoint>& out) { core::DepthFusion f(cs_); f.getElements(out); }
-  bool saveTrajectory(const std::string& path) const { return tracker_.saveTrajectory(path); }
-  // host time of each call SpinOnce makes, and of each call MappingLoopOnce makes (names "mapping.*" inside it)
-  esvo::CallTimes callTimes() const {
-    esvo::CallTimes all = calls_;
-    for (const auto& e : mapper_.calls_.ms) all.ms[e.first] = e.second;
-    return all;
-  }
-
-  const Config& config() const { return cfg_; }
-  std::string status_ = "INITIALIZATION";   // /ESVO_SYSTEM_STATUS
-  std::string error_;
-  std::vector<TickRecord> ticks_;
-  std::vector<MappingRecord> mapping_;
-  esvo::PoseBuffer poses_;
-
- private:
   bool stop(const std::string& why, TickRecord& rec) {
     error_ = why; status_ = "TERMINATE";
     rec.status = status_; ticks_.push_back(rec); ++k_;
