@@ -85,6 +85,13 @@ assert DEPTH_POINT_DTYPE.itemsize == 8 + 8 * (2 + 5 + 1 + 3 + 16)
 EVENT_WIRE_DTYPE = np.dtype([("x", "<u2"), ("y", "<u2"), ("sec", "<u4"), ("nsec", "<u4"), ("polarity", "u1")])
 assert EVENT_WIRE_DTYPE.itemsize == 13
 
+# The 8-counter record of a mapping frame, in the order the C ABI writes it (esvo_fetch_mapping_counters, esvo_results_end)
+MAPPING_COUNTER_KEYS = ("n_events", "n_seeds", "n_solved", "n_culled", "n_fusions", "bm_evals", "lm_evals", "map_size")
+
+
+def _mapping_counters(ctr) -> dict:
+    return dict(zip(MAPPING_COUNTER_KEYS, [int(v) for v in ctr]))
+
 
 def pack_events(x, y, t_ns, pol):
     """SoA events -> wire records (stamp split as ros::Time: sec = t // 1e9, nsec = t % 1e9); pol bytes are kept as given."""
@@ -372,8 +379,7 @@ class Backend:
         self._call("mapping_at_time", self._EV_TYPES + [C.POINTER(C.c_uint64)],
                    _ptr(ex, C.c_uint16), _ptr(ey, C.c_uint16), _ptr(et, C.c_int64), ex.size,
                    _ptr(pt, C.c_int64), _ptr(ps, C.c_double), pt.size, ctr)
-        keys = ["n_events", "n_seeds", "n_solved", "n_culled", "n_fusions", "bm_evals", "lm_evals", "map_size"]
-        return dict(zip(keys, [int(v) for v in ctr]))
+        return _mapping_counters(ctr)
 
     def mapping_reset(self):
         self._call("mapping_reset", [])
@@ -428,8 +434,7 @@ class Backend:
     def fetch_mapping_counters(self):
         ctr = (C.c_uint64 * 8)()
         self._call("fetch_mapping_counters", [C.POINTER(C.c_uint64)], ctr)
-        keys = ["n_events", "n_seeds", "n_solved", "n_culled", "n_fusions", "bm_evals", "lm_evals", "map_size"]
-        return dict(zip(keys, [int(v) for v in ctr]))
+        return _mapping_counters(ctr)
 
     def sgbm_compute(self, left=None, right=None, num_disparities=48, block_size=11, P1=None, P2=None, disp12_max_diff=-1,
                      pre_filter_cap=0, uniqueness_ratio=11):
@@ -497,8 +502,7 @@ class Backend:
         ctr = (C.c_uint64 * 8)()
         self._call("mapping_at_time_selected_dev", [C.POINTER(C.c_int64), C.POINTER(C.c_double), C.c_size_t, C.POINTER(C.c_uint64)],
                    _ptr(pt, C.c_int64), _ptr(ps, C.c_double), pt.size, ctr)
-        keys = ["n_events", "n_seeds", "n_solved", "n_culled", "n_fusions", "bm_evals", "lm_evals", "map_size"]
-        return dict(zip(keys, [int(v) for v in ctr]))
+        return _mapping_counters(ctr)
 
     def init_from_disparity_selected_dev(self, disp16, T_world_left, min_points):
         d = _arr(disp16, np.int16); T = np.ascontiguousarray(T_world_left, np.float64)
@@ -534,21 +538,19 @@ class Backend:
         ctr = (C.c_uint64 * 8)()
         self._call("results_end", [C.c_int64, C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)],
                    int(ticket), out.ctypes.data_as(C.c_void_p), C.byref(n), ctr)
-        keys = ["n_events", "n_seeds", "n_solved", "n_culled", "n_fusions", "bm_evals", "lm_evals", "map_size"]
-        return out[: n.value], dict(zip(keys, [int(v) for v in ctr]))
+        return out[: n.value], _mapping_counters(ctr)
 
     def results_end_view(self, ticket):
         """Zero-copy esvo_results_end: a numpy view of the slot's pinned landing buffer (valid until the slot's next results_begin)."""
         ptr = C.c_void_p(); n = C.c_size_t(0); ctr = (C.c_uint64 * 8)()
         self._call("results_end_view", [C.c_int64, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)],
                    int(ticket), C.byref(ptr), C.byref(n), ctr)
-        keys = ["n_events", "n_seeds", "n_solved", "n_culled", "n_fusions", "bm_evals", "lm_evals", "map_size"]
         if n.value:
             buf = (C.c_char * (n.value * DEPTH_POINT_DTYPE.itemsize)).from_address(ptr.value)
             out = np.frombuffer(buf, dtype=DEPTH_POINT_DTYPE, count=n.value)
         else:
             out = np.zeros(0, DEPTH_POINT_DTYPE)
-        return out, dict(zip(keys, [int(v) for v in ctr]))
+        return out, _mapping_counters(ctr)
 
     def sync(self):
         self._call("sync", [])

@@ -354,35 +354,37 @@ __global__ void __launch_bounds__(kOrdBlock) seeds_order_kernel(DevConsts dc, Bm
 // host launchers
 // --------------------------------------------------------------------------------------------
 int bm_run(Ctx* c) {
-  if (c->n_ev == 0) return ESVO_OK;
+  const SlotBufs& f = c->slot();
+  if (f.n_ev == 0) return ESVO_OK;
   BmArgs a;
-  a.ex = c->d_ex; a.ey = c->d_ey; a.et = c->d_et; a.n = (int)c->n_ev; a.lut = c->d_lut; a.mask = c->d_mask;
-  a.tl = c->obs_ls; a.tr = c->obs_rs; a.pose_t = c->d_pose_t; a.n_poses = (int)c->n_poses; a.out = c->bm;
-  a.counters = (unsigned long long*)c->d_counters;
+  a.ex = f.d_ex; a.ey = f.d_ey; a.et = f.d_et; a.n = (int)f.n_ev; a.lut = c->d_lut; a.mask = c->d_mask;
+  a.tl = f.obs_ls; a.tr = f.obs_rs; a.pose_t = f.d_pose_t; a.n_poses = (int)f.n_poses; a.out = f.bm;
+  a.counters = (unsigned long long*)f.d_counters;
   // TMA-staged strips (faster than per-lane loads, identical results); the per-lane LDG kernel serves step > 1, the up-down
   // rig, very wide searches and a failed tensor-map encode
   const int strip = c->dc.wx + c->dc.dmax - c->dc.dmin + 15;     // + alignment slack of the box origin
   if (c->dc.step == 1 && !c->dc.updown && c->dc.wy <= 8 && strip <= 112 && c->dc.dmax >= c->dc.dmin) {
     CUtensorMap tm;
     const int bw = strip <= 64 ? 64 : 112;
-    if (make_u8_tensor_map(&tm, c->obs_rs, c->dc.W, c->dc.H, c->dc.pitch, bw, c->dc.wy)) {
-      if (bw == 64) bm_tma_kernel<64><<<(int)c->n_ev, 32, 0, c->stream>>>(c->dc, a, tm);
-      else bm_tma_kernel<112><<<(int)c->n_ev, 32, 0, c->stream>>>(c->dc, a, tm);
+    if (make_u8_tensor_map(&tm, f.obs_rs, c->dc.W, c->dc.H, c->dc.pitch, bw, c->dc.wy)) {
+      if (bw == 64) bm_tma_kernel<64><<<(int)f.n_ev, 32, 0, c->stream>>>(c->dc, a, tm);
+      else bm_tma_kernel<112><<<(int)f.n_ev, 32, 0, c->stream>>>(c->dc, a, tm);
       c->launches += 1;
       ESVO_CUDA_TRY(c, cudaGetLastError());
       return ESVO_OK;
     }
   }
-  bm_kernel<<<div_up((int)c->n_ev, BM_WARPS), BM_WARPS * 32, 0, c->stream>>>(c->dc, a);
+  bm_kernel<<<div_up((int)f.n_ev, BM_WARPS), BM_WARPS * 32, 0, c->stream>>>(c->dc, a);
   c->launches += 1;
   ESVO_CUDA_TRY(c, cudaGetLastError());
   return ESVO_OK;
 }
 
 int seeds_order(Ctx* c) {
-  if (c->n_ev == 0) return ESVO_OK;          // counters[1] stays 0 from the frame's memset
-  seeds_order_kernel<<<div_up((int)c->n_ev, kOrdBlock), kOrdBlock, 0, c->stream>>>(c->dc, c->bm, c->d_ex, c->d_ey, c->d_et, c->d_poses, (int)c->n_ev,
-                                                                                 c->d_seeds, (unsigned long long*)c->d_counters);
+  const SlotBufs& f = c->slot();
+  if (f.n_ev == 0) return ESVO_OK;          // counters[1] stays 0 from the frame's memset
+  seeds_order_kernel<<<div_up((int)f.n_ev, kOrdBlock), kOrdBlock, 0, c->stream>>>(c->dc, f.bm, f.d_ex, f.d_ey, f.d_et, f.d_poses, (int)f.n_ev,
+                                                                                f.d_seeds, (unsigned long long*)f.d_counters);
   c->launches += 1;
   ESVO_CUDA_TRY(c, cudaGetLastError());
   return ESVO_OK;

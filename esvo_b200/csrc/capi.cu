@@ -9,8 +9,6 @@
 
 namespace esvo {
 
-template <class T> static cudaError_t dmalloc(T** p, size_t n) { return cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)); }
-
 // 5x5 Gaussian on u8 (cv::GaussianBlur sigma=0: [1 4 6 4 1]/16 per axis, fixed point, round half
 // up, BORDER_REFLECT_101) -- TimeSurfaceObservation::GaussianBlurTS / getTimeSurfaceNegative.
 __device__ __forceinline__ int refl101(int p, int len) {
@@ -41,38 +39,40 @@ __global__ void fp64_probe_kernel(double* out, int iters) {
 }
 
 int smooth_obs(Ctx* c) {
+  SlotBufs& f = c->slot();
   dim3 b(32, 8), g(div_up(c->dc.W, 32), div_up(c->dc.H, 8));
-  c->obs_ls = c->slots[c->cur].own_ls; c->obs_rs = c->slots[c->cur].own_rs;
-  gauss5_u8_kernel<<<g, b, 0, c->stream>>>(c->obs_l, c->obs_ls, c->dc.W, c->dc.H, c->dc.pitch);
-  gauss5_u8_kernel<<<g, b, 0, c->stream>>>(c->obs_r, c->obs_rs, c->dc.W, c->dc.H, c->dc.pitch);
+  f.obs_ls = f.own_ls; f.obs_rs = f.own_rs;
+  gauss5_u8_kernel<<<g, b, 0, c->stream>>>(f.obs_l, f.obs_ls, c->dc.W, c->dc.H, c->dc.pitch);
+  gauss5_u8_kernel<<<g, b, 0, c->stream>>>(f.obs_r, f.obs_rs, c->dc.W, c->dc.H, c->dc.pitch);
   c->launches += 2;
   return ESVO_OK;
 }
 
 int map_alloc_inputs(Ctx* c, size_t n_ev, size_t n_poses) {
-  if (n_ev > c->ev_cap) {
+  SlotBufs& f = c->slot();
+  if (n_ev > f.ev_cap) {
     size_t cap = std::max<size_t>(n_ev, 1024);
-    void* olds[] = {c->bm.flag, c->bm.disp, c->bm.pose_idx, c->bm.cost, c->bm.xrect,
-                    c->d_seeds, c->lm_flag, c->lm_res, c->d_pts};
+    void* olds[] = {f.bm.flag, f.bm.disp, f.bm.pose_idx, f.bm.cost, f.bm.xrect,
+                    f.d_seeds, f.lm_flag, f.lm_res, f.d_pts};
     for (void* p : olds) if (p) cudaFree(p);
-    ESVO_CUDA_TRY(c, dmalloc(&c->bm.flag, cap)); ESVO_CUDA_TRY(c, dmalloc(&c->bm.disp, cap));
-    ESVO_CUDA_TRY(c, dmalloc(&c->bm.pose_idx, cap)); ESVO_CUDA_TRY(c, dmalloc(&c->bm.cost, cap));
-    ESVO_CUDA_TRY(c, dmalloc(&c->bm.xrect, 2 * cap)); ESVO_CUDA_TRY(c, dmalloc(&c->d_seeds, cap));
-    ESVO_CUDA_TRY(c, dmalloc(&c->lm_flag, cap)); ESVO_CUDA_TRY(c, dmalloc(&c->lm_res, 3 * cap));
-    ESVO_CUDA_TRY(c, dmalloc(&c->d_pts, cap));
-    c->ev_cap = cap;
+    ESVO_CUDA_TRY(c, dmalloc(&f.bm.flag, cap)); ESVO_CUDA_TRY(c, dmalloc(&f.bm.disp, cap));
+    ESVO_CUDA_TRY(c, dmalloc(&f.bm.pose_idx, cap)); ESVO_CUDA_TRY(c, dmalloc(&f.bm.cost, cap));
+    ESVO_CUDA_TRY(c, dmalloc(&f.bm.xrect, 2 * cap)); ESVO_CUDA_TRY(c, dmalloc(&f.d_seeds, cap));
+    ESVO_CUDA_TRY(c, dmalloc(&f.lm_flag, cap)); ESVO_CUDA_TRY(c, dmalloc(&f.lm_res, 3 * cap));
+    ESVO_CUDA_TRY(c, dmalloc(&f.d_pts, cap));
+    f.ev_cap = cap;
   }
-  if (n_poses > c->pose_cap) c->pose_cap = std::max<size_t>(n_poses, 256);
-  const size_t need = c->ev_cap * 12 + c->pose_cap * 136 + 64;
-  if (need > c->in_bytes) {
-    if (c->ev_in_valid) { ESVO_CUDA_TRY(c, cudaEventSynchronize(c->ev_in)); c->ev_in_valid = false; }
-    if (c->d_in) { ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream)); cudaFree(c->d_in); }
-    if (c->h_in) cudaFreeHost(c->h_in);
-    ESVO_CUDA_TRY(c, dmalloc(&c->d_in, need));
-    ESVO_CUDA_TRY(c, cudaMallocHost((void**)&c->h_in, need));
-    if (!c->ev_in) ESVO_CUDA_TRY(c, cudaEventCreateWithFlags(&c->ev_in, cudaEventDisableTiming));
-    c->in_bytes = need;
-    c->d_ex = c->d_ey = nullptr; c->d_et = c->d_pose_t = nullptr; c->d_poses = nullptr;
+  if (n_poses > f.pose_cap) f.pose_cap = std::max<size_t>(n_poses, 256);
+  const size_t need = f.ev_cap * 12 + f.pose_cap * 136 + 64;
+  if (need > f.in_bytes) {
+    if (f.ev_in_valid) { ESVO_CUDA_TRY(c, cudaEventSynchronize(f.ev_in)); f.ev_in_valid = false; }
+    if (f.d_in) { ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream)); cudaFree(f.d_in); }
+    if (f.h_in) cudaFreeHost(f.h_in);
+    ESVO_CUDA_TRY(c, dmalloc(&f.d_in, need));
+    ESVO_CUDA_TRY(c, cudaMallocHost((void**)&f.h_in, need));
+    if (!f.ev_in) ESVO_CUDA_TRY(c, cudaEventCreateWithFlags(&f.ev_in, cudaEventDisableTiming));
+    f.in_bytes = need;
+    f.d_ex = f.d_ey = nullptr; f.d_et = f.d_pose_t = nullptr; f.d_poses = nullptr;
   }
   return ESVO_OK;
 }
@@ -82,44 +82,24 @@ int stage_inputs_packed(Ctx* c, const uint16_t* ex, const uint16_t* ey, const in
                         const double* poses, size_t np) {
   int rc = map_alloc_inputs(c, n, np);
   if (rc) return rc;
-  c->n_ev = n; c->n_poses = np;
-  if (c->ev_in_valid) ESVO_CUDA_TRY(c, cudaEventSynchronize(c->ev_in));   // the previous upload from this pinned mirror (long done)
+  SlotBufs& f = c->slot();
+  f.n_ev = n; f.n_poses = np;
+  if (f.ev_in_valid) ESVO_CUDA_TRY(c, cudaEventSynchronize(f.ev_in));   // the previous upload from this pinned mirror (long done)
   const size_t o_et = 0, o_pt = o_et + n * 8, o_ps = o_pt + np * 8, o_ex = o_ps + np * 128, o_ey = o_ex + ((n * 2 + 7) & ~(size_t)7);
   const size_t total = o_ey + n * 2;
-  if (n) { std::memcpy(c->h_in + o_et, et, n * 8); std::memcpy(c->h_in + o_ex, ex, n * 2); std::memcpy(c->h_in + o_ey, ey, n * 2); }
-  if (np) { std::memcpy(c->h_in + o_pt, pt, np * 8); std::memcpy(c->h_in + o_ps, poses, np * 128); }
-  c->d_et = (int64_t*)(c->d_in + o_et); c->d_pose_t = (int64_t*)(c->d_in + o_pt); c->d_poses = (double*)(c->d_in + o_ps);
-  c->d_ex = (uint16_t*)(c->d_in + o_ex); c->d_ey = (uint16_t*)(c->d_in + o_ey);
+  if (n) { std::memcpy(f.h_in + o_et, et, n * 8); std::memcpy(f.h_in + o_ex, ex, n * 2); std::memcpy(f.h_in + o_ey, ey, n * 2); }
+  if (np) { std::memcpy(f.h_in + o_pt, pt, np * 8); std::memcpy(f.h_in + o_ps, poses, np * 128); }
+  f.d_et = (int64_t*)(f.d_in + o_et); f.d_pose_t = (int64_t*)(f.d_in + o_pt); f.d_poses = (double*)(f.d_in + o_ps);
+  f.d_ex = (uint16_t*)(f.d_in + o_ex); f.d_ey = (uint16_t*)(f.d_in + o_ey);
   if (total) {
-    ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->d_in, c->h_in, total, cudaMemcpyHostToDevice, c->stream));
-    ESVO_CUDA_TRY(c, cudaEventRecord(c->ev_in, c->stream));
-    c->ev_in_valid = true;
+    ESVO_CUDA_TRY(c, cudaMemcpyAsync(f.d_in, f.h_in, total, cudaMemcpyHostToDevice, c->stream));
+    ESVO_CUDA_TRY(c, cudaEventRecord(f.ev_in, c->stream));
+    f.ev_in_valid = true;
   }
   return ESVO_OK;
 }
 
-#define SLOT_FIELDS(X) X(obs_l) X(obs_r) X(obs_ls) X(obs_rs) X(ev_cap) X(pose_cap) X(n_ev) X(n_poses) \
-  X(d_ex) X(d_ey) X(d_et) X(d_pose_t) X(d_poses) X(d_in) X(h_in) X(in_bytes) X(ev_in) X(ev_in_valid) X(bm) X(d_seeds) X(lm_flag) X(lm_res) X(d_pts) X(d_counters) \
-  X(h_counters) X(h_pin) X(map)
-void slot_save(Ctx* c) {
-  SlotBufs& s = c->slots[c->cur];
-#define X(f) s.f = c->f;
-  SLOT_FIELDS(X)
-#undef X
-  std::memcpy(s.T_world_left, c->T_world_left, sizeof(s.T_world_left));
-  std::memcpy(s.T_left_world_inv, c->T_left_world_inv, sizeof(s.T_left_world_inv));
-}
-void slot_load(Ctx* c, int i) {
-  SlotBufs& s = c->slots[i];
-#define X(f) c->f = s.f;
-  SLOT_FIELDS(X)
-#undef X
-  std::memcpy(c->T_world_left, s.T_world_left, sizeof(s.T_world_left));
-  std::memcpy(c->T_left_world_inv, s.T_left_world_inv, sizeof(s.T_left_world_inv));
-  c->cur = i;
-  c->stream = s.stream;
-}
-int slot_alloc(Ctx* c, int i) {
+static int slot_alloc(Ctx* c, int i) {
   SlotBufs& s = c->slots[i];
   if (s.allocated) return ESVO_OK;
   const size_t nimg = (size_t)c->dc.pitch * c->dc.H;
@@ -129,7 +109,6 @@ int slot_alloc(Ctx* c, int i) {
   s.obs_ls = s.own_ls; s.obs_rs = s.own_rs;
   ESVO_CUDA_TRY(c, dmalloc(&s.d_counters, kCounters));
   ESVO_CUDA_TRY(c, cudaMallocHost((void**)&s.h_counters, kCounters * 8));
-  ESVO_CUDA_TRY(c, cudaMallocHost((void**)&s.h_pin, 64 * 8));
   ESVO_CUDA_TRY(c, cudaMemset(s.d_counters, 0, kCounters * 8));
   ESVO_CUDA_TRY(c, cudaMemset(s.obs_l, 0, nimg)); ESVO_CUDA_TRY(c, cudaMemset(s.obs_r, 0, nimg));
   ESVO_CUDA_TRY(c, cudaMemset(s.own_ls, 0, nimg)); ESVO_CUDA_TRY(c, cudaMemset(s.own_rs, 0, nimg));
@@ -137,15 +116,32 @@ int slot_alloc(Ctx* c, int i) {
   ESVO_CUDA_TRY(c, cudaEventCreateWithFlags(&s.ev_free, cudaEventDisableTiming));
   ESVO_CUDA_TRY(c, cudaEventCreateWithFlags(&s.ev_pts, cudaEventDisableTiming));
   ESVO_CUDA_TRY(c, cudaEventCreateWithFlags(&s.ev_fuse, cudaEventDisableTiming));
-  {  // the slot's own map / fusion staging
-    MapState* keep = c->map;
-    int rc = fuse_alloc(c);
-    s.map = c->map;
-    c->map = keep;
-    if (rc) return rc;
-  }
+  if (int rc = fuse_alloc(c, &s.map)) return rc;   // the slot's own map / fusion staging
   s.allocated = true;
   return ESVO_OK;
+}
+// Releases everything slot i holds, allocated or partly allocated (the ctx is drained).
+static void slot_free(Ctx* c, int i) {
+  SlotBufs& s = c->slots[i];
+  fuse_free(s.map);
+  s.map = nullptr;
+  void* ps[] = {s.obs_l, s.obs_r, s.own_ls, s.own_rs, s.d_counters, s.d_in, s.bm.flag, s.bm.disp, s.bm.pose_idx, s.bm.cost, s.bm.xrect, s.d_seeds, s.lm_flag, s.lm_res,
+                s.d_pts};
+  for (void* p : ps) if (p) cudaFree(p);
+  if (s.h_counters) cudaFreeHost(s.h_counters);
+  if (s.h_in) cudaFreeHost(s.h_in);
+  if (s.ev_in) cudaEventDestroy(s.ev_in);
+  if (s.ev_obs) cudaEventDestroy(s.ev_obs);
+  if (s.ev_free) cudaEventDestroy(s.ev_free);
+  if (s.ev_pts) cudaEventDestroy(s.ev_pts);
+  if (s.ev_fuse) cudaEventDestroy(s.ev_fuse);
+  if (s.ev_dl) cudaEventDestroy(s.ev_dl);
+  if (s.d_dl) cudaFree(s.d_dl);
+  if (s.d_dl_keys) cudaFree(s.d_dl_keys);
+  if (s.d_dlscal) cudaFree(s.d_dlscal);
+  if (s.h_dlscal) cudaFreeHost(s.h_dlscal);
+  if (s.h_dl) cudaFreeHost(s.h_dl);
+  if (s.stream && s.stream != c->s_main) cudaStreamDestroy(s.stream);
 }
 int drain(Ctx* c) {
   for (int k = 0; k < 2; ++k) if (c->s_tsc[k]) ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->s_tsc[k]));
@@ -177,41 +173,26 @@ static int upload_tables(Ctx* c) {
   return ESVO_OK;
 }
 
-static void rigid_inverse(const double* T, double* I) {
-  for (int i = 0; i < 16; ++i) I[i] = 0;
-  I[15] = 1;
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) I[i * 4 + j] = T[j * 4 + i];
-  for (int i = 0; i < 3; ++i) {
-    double s = 0;
-    for (int k = 0; k < 3; ++k) s += I[i * 4 + k] * T[k * 4 + 3];
-    I[i * 4 + 3] = -s;
-  }
-}
-
-static int stage_mapping(Ctx* c, const uint16_t* ex, const uint16_t* ey, const int64_t* et, size_t n,
-                         const int64_t* pt, const double* poses, size_t np) {
-  return stage_inputs_packed(c, ex, ey, et, n, pt, poses, np);
-}
-
 // The part of esvo_set_ts_pair behind the image copies: the observation pose, and the raw pair as the solver's view of it until
 // createMatchProblem smooths it.
 static int obs_set_pose(Ctx* c, const double T[16]) {
+  SlotBufs& f = c->slot();
   const size_t nimg = (size_t)c->dc.pitch * c->dc.H;
-  std::memcpy(c->T_world_left, T, sizeof(c->T_world_left));
-  rigid_inverse(T, c->T_left_world_inv);
-  if (!c->prm.smooth_time_surface) { c->obs_ls = c->obs_l; c->obs_rs = c->obs_r; }
+  std::memcpy(f.T_world_left, T, sizeof(f.T_world_left));
+  rigid_inverse(T, f.T_left_world_inv);
+  if (!c->prm.smooth_time_surface) { f.obs_ls = f.obs_l; f.obs_rs = f.obs_r; }
   else {
-    ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_ls, c->obs_l, nimg, cudaMemcpyDeviceToDevice, c->stream));
-    ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_rs, c->obs_r, nimg, cudaMemcpyDeviceToDevice, c->stream));
+    ESVO_CUDA_TRY(c, cudaMemcpyAsync(f.obs_ls, f.obs_l, nimg, cudaMemcpyDeviceToDevice, c->stream));
+    ESVO_CUDA_TRY(c, cudaMemcpyAsync(f.obs_rs, f.obs_r, nimg, cudaMemcpyDeviceToDevice, c->stream));
   }
-  ESVO_CUDA_TRY(c, cudaEventRecord(c->slots[c->cur].ev_obs, c->stream));
+  ESVO_CUDA_TRY(c, cudaEventRecord(f.ev_obs, c->stream));
   c->obs_set = true;
   return ESVO_OK;
 }
 
-static int fetch_counters(Ctx* c) {
-  ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->h_counters, c->d_counters, kCounters * 8, cudaMemcpyDeviceToHost, c->stream));
+int fetch_counters(Ctx* c) {
+  SlotBufs& f = c->slot();
+  ESVO_CUDA_TRY(c, cudaMemcpyAsync(f.h_counters, f.d_counters, kCounters * 8, cudaMemcpyDeviceToHost, c->stream));
   ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   return ESVO_OK;
 }
@@ -219,8 +200,6 @@ static int fetch_counters(Ctx* c) {
 }  // namespace esvo
 
 using namespace esvo;
-
-#define CHECK_CTX(c) do { if (!(c)) return ESVO_ERR_INVALID_ARG; cudaSetDevice((c)->device); } while (0)
 
 extern "C" {
 
@@ -262,7 +241,6 @@ ESVO_API int esvo_set_pipeline_depth(esvo_ctx* c, int depth) {
   if (depth < 1 || depth > kMaxSlots) return ESVO_ERR_INVALID_ARG;
   int rc = drain(c);
   if (rc) return rc;
-  slot_save(c);
   if (depth > 1) {
     // The time-surface chain of a frame is ~8 short dependent kernels per camera; with the SMs saturated by the
     // LM kernels of the frames in flight, each of them would queue behind pending LM blocks.  The two cameras get
@@ -278,7 +256,7 @@ ESVO_API int esvo_set_pipeline_depth(esvo_ctx* c, int depth) {
   }
   c->depth = depth;
   c->frame_no = 0;
-  slot_load(c, 0);
+  c->activate(0);
   return ESVO_OK;
 }
 
@@ -333,7 +311,6 @@ ESVO_API esvo_ctx* esvo_create(int device, const esvo_calib* left, const esvo_ca
   c->slots[0].stream = c->s_main;
   const size_t npix = (size_t)d.W * d.H;
   if (slot_alloc(c, 0)) return bail(ESVO_ERR_CUDA);
-  slot_load(c, 0);
   if (dmalloc(&c->d_lut, 2 * npix) || dmalloc(&c->d_mask, npix)) return bail(ESVO_ERR_CUDA);
   for (int cam = 0; cam < 2; ++cam) if (ts_alloc(c, cam)) return bail(ESVO_ERR_CUDA);
   if (upload_tables(c)) return bail(ESVO_ERR_CUDA);
@@ -347,35 +324,13 @@ ESVO_API void esvo_destroy(esvo_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   drain(c);
-  if (c->slots[0].allocated) slot_save(c);
   c->stream = c->s_main;
   for (int cam = 0; cam < 2; ++cam) ts_free(c, cam);
-  for (int i = 0; i < kMaxSlots; ++i) if (c->slots[i].map) { c->map = c->slots[i].map; fuse_free(c); c->slots[i].map = nullptr; }
   track_free(c);
   ew_free(c);
   if (c->d_lut) cudaFree(c->d_lut);
   if (c->d_mask) cudaFree(c->d_mask);
-  for (int i = 0; i < kMaxSlots; ++i) {
-    SlotBufs& s = c->slots[i];
-    void* ps[] = {s.obs_l, s.obs_r, s.own_ls, s.own_rs, s.d_counters, s.d_in, s.bm.flag, s.bm.disp, s.bm.pose_idx, s.bm.cost, s.bm.xrect, s.d_seeds, s.lm_flag, s.lm_res,
-                  s.d_pts};
-    for (void* p : ps) if (p) cudaFree(p);
-    if (s.h_counters) cudaFreeHost(s.h_counters);
-    if (s.h_pin) cudaFreeHost(s.h_pin);
-    if (s.h_in) cudaFreeHost(s.h_in);
-    if (s.ev_in) cudaEventDestroy(s.ev_in);
-    if (s.ev_obs) cudaEventDestroy(s.ev_obs);
-    if (s.ev_free) cudaEventDestroy(s.ev_free);
-    if (s.ev_pts) cudaEventDestroy(s.ev_pts);
-    if (s.ev_fuse) cudaEventDestroy(s.ev_fuse);
-    if (s.ev_dl) cudaEventDestroy(s.ev_dl);
-    if (s.d_dl) cudaFree(s.d_dl);
-    if (s.d_dl_keys) cudaFree(s.d_dl_keys);
-    if (s.d_dlscal) cudaFree(s.d_dlscal);
-    if (s.h_dlscal) cudaFreeHost(s.h_dlscal);
-    if (s.h_dl) cudaFreeHost(s.h_dl);
-    if (s.stream && s.stream != c->s_main) cudaStreamDestroy(s.stream);
-  }
+  for (int i = 0; i < kMaxSlots; ++i) slot_free(c, i);
   for (auto& f : c->win) { cudaFree(f.pts); cudaFree(f.cnt); if (f.last_read) cudaEventDestroy(f.last_read); }
   for (auto& f : c->win_pool) { cudaFree(f.pts); cudaFree(f.cnt); if (f.last_read) cudaEventDestroy(f.last_read); }
   for (auto e : c->prof_pool) cudaEventDestroy(e);
@@ -384,7 +339,6 @@ ESVO_API void esvo_destroy(esvo_ctx* c) {
   if (c->hist.ev_join) cudaEventDestroy(c->hist.ev_join);
   for (void* p : {(void*)c->pub.xyz, (void*)c->pub.sorted, (void*)c->pub.d_scal}) if (p) cudaFree(p);
   if (c->pub.h_scal) cudaFreeHost(c->pub.h_scal);
-  if (c->h_stage) cudaFreeHost(c->h_stage);
   for (int k = 0; k < 2; ++k) if (c->s_tsc[k] && c->s_tsc[k] != c->s_main) cudaStreamDestroy(c->s_tsc[k]);
   if (c->ev_ts_join) cudaEventDestroy(c->ev_ts_join);
   if (c->s_copy) cudaStreamDestroy(c->s_copy);
@@ -521,17 +475,18 @@ ESVO_API int esvo_set_ts_pair(esvo_ctx* c, const uint8_t* l, const uint8_t* r, c
   CHECK_CTX(c);
   if (!T) return ESVO_ERR_INVALID_ARG;
   { int rc0 = drain(c); if (rc0) return rc0; }
+  SlotBufs& f = c->slot();
   const DevConsts& d = c->dc;
   const size_t nimg = (size_t)d.pitch * d.H;
-  if (l) ESVO_CUDA_TRY(c, cudaMemcpy2DAsync(c->obs_l, d.pitch, l, d.W, d.W, d.H, cudaMemcpyHostToDevice, c->stream));
+  if (l) ESVO_CUDA_TRY(c, cudaMemcpy2DAsync(f.obs_l, d.pitch, l, d.W, d.W, d.H, cudaMemcpyHostToDevice, c->stream));
   else {
     if (!c->ts[0].built) { c->set_error("ts_left == NULL but no time surface was built for camera 0"); return ESVO_ERR_STATE; }
-    if (c->obs_l != c->ts[0].last_img) ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_l, c->ts[0].last_img, nimg, cudaMemcpyDeviceToDevice, c->stream));
+    if (f.obs_l != c->ts[0].last_img) ESVO_CUDA_TRY(c, cudaMemcpyAsync(f.obs_l, c->ts[0].last_img, nimg, cudaMemcpyDeviceToDevice, c->stream));
   }
-  if (r) ESVO_CUDA_TRY(c, cudaMemcpy2DAsync(c->obs_r, d.pitch, r, d.W, d.W, d.H, cudaMemcpyHostToDevice, c->stream));
+  if (r) ESVO_CUDA_TRY(c, cudaMemcpy2DAsync(f.obs_r, d.pitch, r, d.W, d.W, d.H, cudaMemcpyHostToDevice, c->stream));
   else {
     if (!c->ts[1].built) { c->set_error("ts_right == NULL but no time surface was built for camera 1"); return ESVO_ERR_STATE; }
-    if (c->obs_r != c->ts[1].last_img) ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_r, c->ts[1].last_img, nimg, cudaMemcpyDeviceToDevice, c->stream));
+    if (f.obs_r != c->ts[1].last_img) ESVO_CUDA_TRY(c, cudaMemcpyAsync(f.obs_r, c->ts[1].last_img, nimg, cudaMemcpyDeviceToDevice, c->stream));
   }
   int rc = obs_set_pose(c, T);
   if (rc) return rc;
@@ -586,7 +541,7 @@ ESVO_API int esvo_ts_history_store_dev(esvo_ctx* c, int64_t stamp) {
 ESVO_API int esvo_set_ts_pair_stored_dev(esvo_ctx* c, int64_t stamp, const double T[16]) {
   CHECK_CTX(c);
   if (!T) return ESVO_ERR_INVALID_ARG;
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   Ctx::TsHistory& h = c->hist;
   size_t i = h.cap();
   for (size_t k = 0; k < h.cap(); ++k) if (h.used[k] && h.stamp[k] == stamp) { i = k; break; }
@@ -594,10 +549,11 @@ ESVO_API int esvo_set_ts_pair_stored_dev(esvo_ctx* c, int64_t stamp, const doubl
     c->set_error("esvo_set_ts_pair_stored_dev: no time-surface pair is stored under stamp " + std::to_string((long long)stamp));
     return ESVO_ERR_STATE;
   }
+  SlotBufs& f = c->slot();
   const size_t nimg = (size_t)c->dc.pitch * c->dc.H;
   ESVO_CUDA_TRY(c, cudaStreamWaitEvent(c->stream, h.ev[i], 0));
-  ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_l, h.buf + 2 * i * nimg, nimg, cudaMemcpyDeviceToDevice, c->stream));
-  ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->obs_r, h.buf + (2 * i + 1) * nimg, nimg, cudaMemcpyDeviceToDevice, c->stream));
+  ESVO_CUDA_TRY(c, cudaMemcpyAsync(f.obs_l, h.buf + 2 * i * nimg, nimg, cudaMemcpyDeviceToDevice, c->stream));
+  ESVO_CUDA_TRY(c, cudaMemcpyAsync(f.obs_r, h.buf + (2 * i + 1) * nimg, nimg, cudaMemcpyDeviceToDevice, c->stream));
   ESVO_CUDA_TRY(c, cudaEventRecord(h.ev[i], c->stream));
   return obs_set_pose(c, T);
 }
@@ -607,9 +563,8 @@ ESVO_API int esvo_set_ts_pair_dev(esvo_ctx* c, const double T[16]) {
   if (!T) return ESVO_ERR_INVALID_ARG;
   if (!c->ts[0].built || !c->ts[1].built) { c->set_error("esvo_set_ts_pair_dev needs a built time surface for both cameras"); return ESVO_ERR_STATE; }
   // begin a new frame: rotate to the next pipeline slot
-  slot_save(c);
-  slot_load(c, (int)(c->frame_no % (uint64_t)c->depth));
-  SlotBufs& sl = c->slots[c->cur];
+  c->activate((int)(c->frame_no % (uint64_t)c->depth));
+  SlotBufs& sl = c->slot();
   // Hand the two freshly built images to the slot WITHOUT copying: swap the slot's observation buffers with
   // the time-surface output buffers.  The buffers the TS state receives in exchange are overwritten by the
   // next build, so the TS stream must first wait until the slot's previous frame stopped reading them.
@@ -625,20 +580,20 @@ ESVO_API int esvo_set_ts_pair_dev(esvo_ctx* c, const double T[16]) {
   for (int cam = 0; cam < 2; ++cam) {
     TsState& t = c->ts[cam];
     if (t.last_img != t.img_out) { c->set_error("esvo_set_ts_pair_dev: time surface not rebuilt since the last hand-off"); return ESVO_ERR_STATE; }
-    uint8_t*& mine = cam == 0 ? c->obs_l : c->obs_r;
+    uint8_t*& mine = cam == 0 ? sl.obs_l : sl.obs_r;
     std::swap(mine, t.img_out);
     t.last_img = mine;
   }
-  if (!c->prm.smooth_time_surface) { c->obs_ls = c->obs_l; c->obs_rs = c->obs_r; }   // otherwise smooth_obs() fills obs_ls/obs_rs
-  std::memcpy(c->T_world_left, T, sizeof(c->T_world_left));
-  rigid_inverse(T, c->T_left_world_inv);     // travels to the LM kernel by value: no upload, nothing pinned to guard
+  if (!c->prm.smooth_time_surface) { sl.obs_ls = sl.obs_l; sl.obs_rs = sl.obs_r; }   // otherwise smooth_obs() fills obs_ls/obs_rs
+  std::memcpy(sl.T_world_left, T, sizeof(sl.T_world_left));
+  rigid_inverse(T, sl.T_left_world_inv);     // travels to the LM kernel by value: no upload, nothing pinned to guard
   c->obs_set = true;
   return ESVO_OK;
 }
 
 static int run_bm_stage(esvo_ctx* c) {
   if (c->prm.smooth_time_surface) { int rc = smooth_obs(c); if (rc) return rc; }  // EventBM.cpp:68-72
-  ESVO_CUDA_TRY(c, cudaMemsetAsync(c->d_counters, 0, kCounters * 8, c->stream));
+  ESVO_CUDA_TRY(c, cudaMemsetAsync(c->slot().d_counters, 0, kCounters * 8, c->stream));
   cudaEvent_t pe = c->prof_begin(1);
   int rc = bm_run(c);
   c->prof_end(pe);
@@ -650,17 +605,18 @@ ESVO_API int esvo_bm_match(esvo_ctx* c, const uint16_t* ex, const uint16_t* ey, 
                            const int64_t* pt, const double* poses, size_t np, esvo_seed* out, size_t* n_seeds,
                            uint64_t* n_evals) {
   CHECK_CTX(c);
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   if (!c->obs_set) return ESVO_ERR_STATE;
   if (!n_seeds || (n && (!ex || !ey || !et))) return ESVO_ERR_INVALID_ARG;
-  int rc = stage_mapping(c, ex, ey, et, n, pt, poses, np);
+  int rc = stage_inputs_packed(c, ex, ey, et, n, pt, poses, np);
   if (rc) return rc;
   if ((rc = run_bm_stage(c))) return rc;
   if ((rc = fetch_counters(c))) return rc;
-  const size_t cnt = (size_t)c->h_counters[1];
-  if (n_evals) *n_evals = c->h_counters[5];
+  const SlotBufs& f = c->slot();
+  const size_t cnt = (size_t)f.h_counters[1];
+  if (n_evals) *n_evals = f.h_counters[5];
   if (cnt > *n_seeds) { *n_seeds = cnt; return ESVO_ERR_CAPACITY; }
-  if (cnt) ESVO_CUDA_TRY(c, cudaMemcpy(out, c->d_seeds, cnt * sizeof(esvo_seed), cudaMemcpyDeviceToHost));
+  if (cnt) ESVO_CUDA_TRY(c, cudaMemcpy(out, f.d_seeds, cnt * sizeof(esvo_seed), cudaMemcpyDeviceToHost));
   *n_seeds = cnt;
   return ESVO_OK;
 }
@@ -669,22 +625,23 @@ ESVO_API int esvo_bm_match(esvo_ctx* c, const uint16_t* ex, const uint16_t* ey, 
 ESVO_API int esvo_depth_solve(esvo_ctx* c, const esvo_seed* seeds, size_t n, esvo_depth_point* out, size_t* n_out,
                               uint64_t* n_evals) {
   CHECK_CTX(c);
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   if (!c->obs_set) return ESVO_ERR_STATE;
   if (!n_out || (n && !seeds)) return ESVO_ERR_INVALID_ARG;
   if (n == 0) { *n_out = 0; if (n_evals) *n_evals = 0; return ESVO_OK; }
-  int rc = map_alloc_inputs(c, std::max(n, c->n_ev), c->n_poses);
+  SlotBufs& f = c->slot();
+  int rc = map_alloc_inputs(c, std::max(n, f.n_ev), f.n_poses);
   if (rc) return rc;
-  ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->d_seeds, seeds, n * sizeof(esvo_seed), cudaMemcpyHostToDevice, c->stream));
-  ESVO_CUDA_TRY(c, cudaMemsetAsync(c->d_counters, 0, kCounters * 8, c->stream));
-  { cudaEvent_t pe = c->prof_begin(3); rc = lm_run(c, c->d_seeds, n); c->prof_end(pe); }
+  ESVO_CUDA_TRY(c, cudaMemcpyAsync(f.d_seeds, seeds, n * sizeof(esvo_seed), cudaMemcpyHostToDevice, c->stream));
+  ESVO_CUDA_TRY(c, cudaMemsetAsync(f.d_counters, 0, kCounters * 8, c->stream));
+  { cudaEvent_t pe = c->prof_begin(3); rc = lm_run(c, f.d_seeds, n); c->prof_end(pe); }
   if (rc) return rc;
-  if ((rc = points_order_impl(c, c->d_seeds, n, 0, 0, 0, 0, 0, nullptr, nullptr))) return rc;
+  if ((rc = points_order_impl(c, f.d_seeds, n, 0, 0, 0, 0, 0, nullptr, nullptr))) return rc;
   if ((rc = fetch_counters(c))) return rc;
-  const size_t cnt = (size_t)c->h_counters[3];
-  if (n_evals) *n_evals = c->h_counters[6];
+  const size_t cnt = (size_t)f.h_counters[3];
+  if (n_evals) *n_evals = f.h_counters[6];
   if (cnt > *n_out) { *n_out = cnt; return ESVO_ERR_CAPACITY; }
-  if (cnt) ESVO_CUDA_TRY(c, cudaMemcpy(out, c->d_pts, cnt * sizeof(esvo_depth_point), cudaMemcpyDeviceToHost));
+  if (cnt) ESVO_CUDA_TRY(c, cudaMemcpy(out, f.d_pts, cnt * sizeof(esvo_depth_point), cudaMemcpyDeviceToHost));
   *n_out = cnt;
   return ESVO_OK;
 }

@@ -13,8 +13,6 @@ int fuse_reserve(Ctx* c, size_t total_points);
 int fuse_window(Ctx* c, const Ctx::WinFrame* frames, int nframes, int radius);
 int sgbm_run(Ctx* c, const uint8_t* d_left, const uint8_t* d_right, int pitch, const esvo_sgbm::Dims& dm, int16_t* d_out);
 
-template <class T> static cudaError_t dmalloc(T** p, size_t n) { return cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)); }
-
 // Window vectors are recycled through a FIFO pool.  A vector popped from the window may still be read by the
 // fusion of the frame that preceded the pop (running on another slot's stream), so it carries an event recorded
 // behind that fusion, and it is only reused after `depth` further frames: the wait below is then already satisfied.
@@ -43,21 +41,15 @@ static int win_retire(Ctx* c, Ctx::WinFrame f) {
   return ESVO_OK;
 }
 
-static int fetch_counters2(Ctx* c) {
-  ESVO_CUDA_TRY(c, cudaMemcpyAsync(c->h_counters, c->d_counters, kCounters * 8, cudaMemcpyDeviceToHost, c->stream));
-  ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
-  return ESVO_OK;
-}
-
 // esvo_Mapping::MappingAtTime (esvo_Mapping.cpp:261-399), kernels only, everything stays on the device.
 static int run_mapping_frame(Ctx* c) {
   const esvo_params& p = c->prm;
   int rc;
-  SlotBufs& sl = c->slots[c->cur];
+  SlotBufs& sl = c->slot();
   ESVO_CUDA_TRY(c, cudaStreamWaitEvent(c->stream, sl.ev_obs, 0));        // observation of this frame is in place
   cudaEvent_t pe = c->prof_begin(1);
   if (p.smooth_time_surface && (rc = smooth_obs(c))) return rc;           // createMatchProblem (EventBM.cpp:68-72)
-  ESVO_CUDA_TRY(c, cudaMemsetAsync(c->d_counters, 0, kCounters * 8, c->stream));
+  ESVO_CUDA_TRY(c, cudaMemsetAsync(sl.d_counters, 0, kCounters * 8, c->stream));
   if ((rc = bm_run(c))) return rc;                                        // :308-309
   c->prof_end(pe); pe = c->prof_begin(2);
   if ((rc = seeds_order(c))) return rc;
@@ -65,15 +57,15 @@ static int run_mapping_frame(Ctx* c) {
   // (Giving the LM kernel its own low-priority stream and the short stages high-priority streams made the pipeline
   //  slower and erratic when it was tried, so everything of a frame stays on the slot's single stream.)
   pe = c->prof_begin(3);
-  if ((rc = lm_run(c, c->d_seeds, 0))) return rc;                         // :330
+  if ((rc = lm_run(c, sl.d_seeds, 0))) return rc;                         // :330
   c->prof_end(pe);
   ESVO_CUDA_TRY(c, cudaEventRecord(sl.ev_free, c->stream));               // the slot's observation buffers are free again
   sl.ev_free_valid = true;
   Ctx::WinFrame f;
-  if ((rc = win_acquire(c, std::max<size_t>(c->n_ev, 1), f))) return rc;
+  if ((rc = win_acquire(c, std::max<size_t>(sl.n_ev, 1), f))) return rc;
   const double cost_thr = p.residual_vis_threshold * p.residual_vis_threshold * (double)(p.patch_size_x * p.patch_size_y);
   pe = c->prof_begin(4);
-  if ((rc = points_order_impl(c, c->d_seeds, 0, 1, p.stdvar_vis_threshold, cost_thr, p.invdepth_min_range,
+  if ((rc = points_order_impl(c, sl.d_seeds, 0, 1, p.stdvar_vis_threshold, cost_thr, p.invdepth_min_range,
                               p.invdepth_max_range, f.pts, f.cnt)))       // :334 pointCulling
     return rc;
   c->prof_end(pe);
@@ -113,7 +105,7 @@ static int run_mapping_frame(Ctx* c) {
   ESVO_CUDA_TRY(c, cudaEventRecord(sl.ev_pts, c->stream));
   sl.ev_pts_valid = true;
   pe = c->prof_begin(5);
-  if ((rc = fuse_reset_map(c, c->T_world_left))) return rc;               // :268-272 fresh DepthFrame at the obs pose
+  if ((rc = fuse_reset_map(c, sl.T_world_left))) return rc;               // :268-272 fresh DepthFrame at the obs pose
   {  // size the staging area once for a full window so that steady-state frames never reallocate
     size_t tot = 0, mx = 0;
     for (auto& w : c->win) { tot += w.cap; mx = std::max(mx, w.cap); }
@@ -144,38 +136,55 @@ static int run_mapping_frame(Ctx* c) {
   return rc;
 }
 
+// The 8-counter record of a mapping frame {n_events, n_seeds, n_solved, n_culled, n_fusions, bm_evals, lm_evals, map_size}
+// from the slot's fetched counters and its map scalars (fuse_fetch_scalars: [0] = n_fusions, [2] = map size).
+static void mapping_counters(const SlotBufs& s, const unsigned long long map_scal[4], uint64_t out[8]) {
+  out[0] = s.n_ev; out[1] = s.h_counters[1]; out[2] = s.h_counters[2]; out[3] = s.h_counters[3];
+  out[4] = map_scal[0]; out[5] = s.h_counters[5]; out[6] = s.h_counters[6]; out[7] = map_scal[2];
+}
 static int fetch_mapping_counters(Ctx* c, uint64_t out[8]) {
-  int rc = fetch_counters2(c);
+  int rc = fetch_counters(c);
   if (rc) return rc;
   unsigned long long sc[4];
   if ((rc = fuse_fetch_scalars(c, sc))) return rc;
-  out[0] = c->n_ev; out[1] = c->h_counters[1]; out[2] = c->h_counters[2]; out[3] = c->h_counters[3];
-  out[4] = sc[0]; out[5] = c->h_counters[5]; out[6] = c->h_counters[6]; out[7] = sc[2];
+  mapping_counters(c->slot(), sc, out);
   return ESVO_OK;
+}
+// The slot holding results_begin's ticket, once its hand-off has landed.  Slots need not rotate (the host esvo_set_ts_pair
+// keeps one), so every slot is searched.
+static int ticket_slot(Ctx* c, int64_t ticket, const char* who, SlotBufs** out) {
+  for (SlotBufs& s : c->slots)
+    if (s.dl_ticket == ticket) {
+      ESVO_CUDA_TRY(c, cudaEventSynchronize(s.ev_dl));
+      *out = &s;
+      return ESVO_OK;
+    }
+  c->set_error(std::string(who) + ": unknown ticket");
+  return ESVO_ERR_STATE;
 }
 }  // namespace esvo
 
 using namespace esvo;
-#define CHECK_CTX(c) do { if (!(c)) return ESVO_ERR_INVALID_ARG; cudaSetDevice((c)->device); } while (0)
 
 extern "C" {
 
 ESVO_API int esvo_depth_cull(esvo_ctx* c, esvo_depth_point* pts, size_t* n, double std_thr, double cost_thr,
                              double rmin, double rmax) {
   CHECK_CTX(c);
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   if (!n || (*n && !pts)) return ESVO_ERR_INVALID_ARG;
   if (*n == 0) return ESVO_OK;
-  int rc = map_alloc_inputs(c, std::max(*n, c->n_ev), c->n_poses);
+  SlotBufs& f = c->slot();
+  int rc = map_alloc_inputs(c, std::max(*n, f.n_ev), f.n_poses);
   if (rc) return rc;
   esvo_depth_point* tmp = nullptr;
   ESVO_CUDA_TRY(c, dmalloc(&tmp, *n));
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(tmp, pts, *n * sizeof(esvo_depth_point), cudaMemcpyHostToDevice, c->stream));
   rc = cull_points(c, tmp, *n, std_thr, cost_thr, rmin, rmax);
-  if (!rc) rc = fetch_counters2(c);
+  if (!rc) rc = fetch_counters(c);
   if (!rc) {
-    const size_t cnt = (size_t)c->h_counters[3];
-    if (cnt) cudaMemcpy(pts, c->d_pts, cnt * sizeof(esvo_depth_point), cudaMemcpyDeviceToHost);
+    const size_t cnt = (size_t)f.h_counters[3];
+    if (cnt) cudaMemcpy(pts, f.d_pts, cnt * sizeof(esvo_depth_point), cudaMemcpyDeviceToHost);
     *n = cnt;
   }
   cudaFree(tmp);
@@ -185,7 +194,7 @@ ESVO_API int esvo_depth_cull(esvo_ctx* c, esvo_depth_point* pts, size_t* n, doub
 ESVO_API int esvo_fuse(esvo_ctx* c, const esvo_depth_point* pts, size_t n, const double T[16], int radius, int reset_map,
                        int* n_fusions) {
   CHECK_CTX(c);
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   if (n && !pts) return ESVO_ERR_INVALID_ARG;
   int rc;
   if (reset_map) { if (!T) return ESVO_ERR_INVALID_ARG; if ((rc = fuse_reset_map(c, T))) return rc; }
@@ -225,7 +234,7 @@ ESVO_API int esvo_seeds_to_points(esvo_ctx* c, const esvo_seed* seeds, size_t n,
 }
 ESVO_API int esvo_naive_propagate(esvo_ctx* c, const esvo_depth_point* pts, size_t n, const double T[16], int reset_map) {
   CHECK_CTX(c);
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   if (n && !pts) return ESVO_ERR_INVALID_ARG;
   int rc = ESVO_OK;
   if (reset_map) { if (!T) return ESVO_ERR_INVALID_ARG; if ((rc = fuse_reset_map(c, T))) return rc; }
@@ -244,20 +253,20 @@ ESVO_API int esvo_naive_propagate(esvo_ctx* c, const esvo_depth_point* pts, size
 
 ESVO_API int esvo_map_clean(esvo_ctx* c, double var_thr, double age_thr, double rmax, double rmin) {
   CHECK_CTX(c);
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   return map_clean(c, var_thr, age_thr, rmax, rmin);
 }
-ESVO_API int esvo_map_regularize(esvo_ctx* c) { CHECK_CTX(c); if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; } return map_regularize(c); }
+ESVO_API int esvo_map_regularize(esvo_ctx* c) { CHECK_CTX(c); if (int rc0 = drain_if_pipelined(c)) return rc0; return map_regularize(c); }
 ESVO_API int esvo_map_download(esvo_ctx* c, esvo_depth_point* out, size_t* n) {
   CHECK_CTX(c);
   if (!n) return ESVO_ERR_INVALID_ARG;
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   return map_download(c, out, n);
 }
 ESVO_API int esvo_map_publish_dev(esvo_ctx* c, const double T[16], int64_t stamp, size_t* n_points) {
   CHECK_CTX(c);
   if (!T || !n_points) return ESVO_ERR_INVALID_ARG;
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   c->pub.valid = false;
   int rc = map_publish(c, T, n_points);
   if (rc) return rc;
@@ -299,7 +308,7 @@ ESVO_API int esvo_sgbm_compute(esvo_ctx* c, const uint8_t* left, const uint8_t* 
     src_l = d_l; src_r = d_r; pitch = W;
   } else {                                                         // the observation pair that is already on the device
     if (!c->obs_set) { cleanup(); return ESVO_ERR_STATE; }
-    src_l = c->obs_l; src_r = c->obs_r; pitch = c->dc.pitch;
+    src_l = c->slot().obs_l; src_r = c->slot().obs_r; pitch = c->dc.pitch;
   }
   int rc = sgbm_run(c, src_l, src_r, pitch, dm, d_out);
   if (rc == ESVO_OK && cudaMemcpy(disp16_out, d_out, (size_t)W * H * 2, cudaMemcpyDeviceToHost) != cudaSuccess) rc = ESVO_ERR_CUDA;
@@ -341,7 +350,7 @@ static int init_from_disparity(esvo_ctx* c, const int16_t* disp16, const uint16_
     return ESVO_OK;
   }
   c->win.push_back(f);                                             // :485 dqvDepthPoints_.push_back(vdp_sgm)
-  std::memcpy(c->T_world_left, T, sizeof(c->T_world_left));
+  std::memcpy(c->slot().T_world_left, T, sizeof(SlotBufs::T_world_left));
   if ((rc = fuse_zero_fusion_counter(c))) return rc;
   if ((rc = fuse_points(c, f.pts, (size_t)cnt, nullptr, 0, /*naive=*/1))) return rc;   // :486 naive_propagation
   if ((rc = fuse_finish(c, true))) return rc;
@@ -398,7 +407,8 @@ ESVO_API int esvo_mapping_at_time_selected_dev(esvo_ctx* c, const int64_t* pt, c
   int rc = map_alloc_inputs(c, w.n, np);
   if (rc) return rc;
   if ((rc = stage_inputs_packed(c, nullptr, nullptr, nullptr, 0, pt, poses, np))) return rc;   // the poses only
-  c->n_ev = w.n; c->d_ex = w.kx; c->d_ey = w.ky; c->d_et = w.kt;                                // the events in place
+  SlotBufs& f = c->slot();
+  f.n_ev = w.n; f.d_ex = w.kx; f.d_ey = w.ky; f.d_et = w.kt;                                      // the events in place
   if ((rc = esvo_run_mapping(c))) return rc;
   uint64_t ctr[8];
   if ((rc = fetch_mapping_counters(c, ctr))) return rc;
@@ -454,17 +464,17 @@ ESVO_API int esvo_stage_mapping_inputs_dev(esvo_ctx* c, const uint16_t* ex, cons
   if (np && (!pt || !poses)) return ESVO_ERR_INVALID_ARG;
   int rc = map_alloc_inputs(c, n, np);
   if (rc) return rc;
-  c->n_ev = n; c->n_poses = np;
-  c->d_ex = const_cast<uint16_t*>(ex); c->d_ey = const_cast<uint16_t*>(ey); c->d_et = const_cast<int64_t*>(et);
-  c->d_pose_t = const_cast<int64_t*>(pt); c->d_poses = const_cast<double*>(poses);
+  SlotBufs& f = c->slot();
+  f.n_ev = n; f.n_poses = np;
+  f.d_ex = const_cast<uint16_t*>(ex); f.d_ey = const_cast<uint16_t*>(ey); f.d_et = const_cast<int64_t*>(et);
+  f.d_pose_t = const_cast<int64_t*>(pt); f.d_poses = const_cast<double*>(poses);
   return ESVO_OK;
 }
 // ---- asynchronous result hand-off for pipelined operation ----
 ESVO_API int esvo_results_begin(esvo_ctx* c, int64_t* ticket_out) {
   CHECK_CTX(c);
   if (c->frame_no == 0) return ESVO_ERR_STATE;
-  slot_save(c);
-  SlotBufs& sl = c->slots[c->cur];
+  SlotBufs& sl = c->slot();
   if (sl.dl_ticket >= 0) { c->set_error("esvo_results_begin: the previous results of this pipeline slot were not collected"); return ESVO_ERR_STATE; }
   const size_t npix = (size_t)c->dc.W * c->dc.H;
   if (!sl.d_dl) {
@@ -495,21 +505,15 @@ ESVO_API int esvo_results_begin(esvo_ctx* c, int64_t* ticket_out) {
 ESVO_API int esvo_results_end(esvo_ctx* c, int64_t ticket, esvo_depth_point* out, size_t* n, uint64_t counters[8]) {
   CHECK_CTX(c);
   if (!n || ticket < 0) return ESVO_ERR_INVALID_ARG;
-  int si = -1;
-  for (int i = 0; i < kMaxSlots; ++i) if (c->slots[i].dl_ticket == ticket) { si = i; break; }   // slots need not rotate (host esvo_set_ts_pair keeps one)
-  if (si < 0) { c->set_error("esvo_results_end: unknown ticket"); return ESVO_ERR_STATE; }
-  SlotBufs& sl = c->slots[si];
-  ESVO_CUDA_TRY(c, cudaEventSynchronize(sl.ev_dl));
-  const size_t cnt = (size_t)sl.h_dlscal[1];
-  if (counters) {
-    counters[0] = sl.n_ev; counters[1] = sl.h_counters[1]; counters[2] = sl.h_counters[2]; counters[3] = sl.h_counters[3];
-    counters[4] = sl.h_dlscal[4]; counters[5] = sl.h_counters[5]; counters[6] = sl.h_counters[6]; counters[7] = sl.h_dlscal[6];
-  }
+  SlotBufs* sl;
+  if (int rc = ticket_slot(c, ticket, "esvo_results_end", &sl)) return rc;
+  const size_t cnt = (size_t)sl->h_dlscal[1];
+  if (counters) mapping_counters(*sl, sl->h_dlscal + 4, counters);
   if (cnt > *n) { *n = cnt; return ESVO_ERR_CAPACITY; }
   if (cnt && !out) return ESVO_ERR_INVALID_ARG;
-  std::memcpy(out, sl.h_dl, cnt * sizeof(esvo_depth_point));   // already in SmartGrid list order (creation sequence)
+  std::memcpy(out, sl->h_dl, cnt * sizeof(esvo_depth_point));   // already in SmartGrid list order (creation sequence)
   *n = cnt;
-  sl.dl_ticket = -1;
+  sl->dl_ticket = -1;
   return ESVO_OK;
 }
 // Zero-copy form: *out points into the slot's pinned landing buffer (written by the gather kernel over PCIe); valid until the
@@ -517,21 +521,15 @@ ESVO_API int esvo_results_end(esvo_ctx* c, int64_t ticket, esvo_depth_point* out
 ESVO_API int esvo_results_end_view(esvo_ctx* c, int64_t ticket, const esvo_depth_point** out, size_t* n, uint64_t counters[8]) {
   CHECK_CTX(c);
   if (!n || !out || ticket < 0) return ESVO_ERR_INVALID_ARG;
-  int si = -1;
-  for (int i = 0; i < kMaxSlots; ++i) if (c->slots[i].dl_ticket == ticket) { si = i; break; }
-  if (si < 0) { c->set_error("esvo_results_end_view: unknown ticket"); return ESVO_ERR_STATE; }
-  SlotBufs& sl = c->slots[si];
-  ESVO_CUDA_TRY(c, cudaEventSynchronize(sl.ev_dl));
-  if (counters) {
-    counters[0] = sl.n_ev; counters[1] = sl.h_counters[1]; counters[2] = sl.h_counters[2]; counters[3] = sl.h_counters[3];
-    counters[4] = sl.h_dlscal[4]; counters[5] = sl.h_counters[5]; counters[6] = sl.h_counters[6]; counters[7] = sl.h_dlscal[6];
-  }
-  *out = (const esvo_depth_point*)sl.h_dl;
-  *n = (size_t)sl.h_dlscal[1];
-  sl.dl_ticket = -1;
+  SlotBufs* sl;
+  if (int rc = ticket_slot(c, ticket, "esvo_results_end_view", &sl)) return rc;
+  if (counters) mapping_counters(*sl, sl->h_dlscal + 4, counters);
+  *out = (const esvo_depth_point*)sl->h_dl;
+  *n = (size_t)sl->h_dlscal[1];
+  sl->dl_ticket = -1;
   return ESVO_OK;
 }
-ESVO_API uint64_t esvo_debug_counter(esvo_ctx* c, int idx) { return (c && idx >= 0 && idx < kCounters) ? c->h_counters[idx] : 0; }
+ESVO_API uint64_t esvo_debug_counter(esvo_ctx* c, int idx) { return (c && idx >= 0 && idx < kCounters) ? c->slot().h_counters[idx] : 0; }
 ESVO_API int esvo_profile(esvo_ctx* c, int stage_mask) {
   CHECK_CTX(c);
   c->prof = (unsigned)stage_mask & 0xffu;

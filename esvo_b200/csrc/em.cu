@@ -291,8 +291,9 @@ int em_match(Ctx* c, const esvo_em_params* prm, const uint16_t* lx, const uint16
   a.lx = dlx; a.ly = dly; a.lt = dlt; a.lp = dlp; a.n = (int)total; a.slice_of = dso; a.slice_poses = dposes;
   a.rx = drx; a.ry = dry; a.rt = drt; a.rp = drp; a.nr = (int)nr;
   a.lut_l = c->d_lut; a.lut_r = dlut_r;
-  a.tl = c->obs_l; a.tr = c->obs_r;      // EventMatcher::createMatchProblem does not smooth the observation (:51-58)
-  std::memcpy(a.T_left_world, c->T_left_world_inv, sizeof(a.T_left_world));
+  const SlotBufs& f = c->slot();
+  a.tl = f.obs_l; a.tr = f.obs_r;      // EventMatcher::createMatchProblem does not smooth the observation (:51-58)
+  std::memcpy(a.T_left_world, f.T_left_world_inv, sizeof(a.T_left_world));
   a.time_thr = prm->time_threshold_s; a.epi_thr = prm->epipolar_threshold; a.ncc_thr = prm->ts_ncc_threshold;
   a.wx = prm->patch_size_x; a.wy = prm->patch_size_y; a.NT = prm->num_thread < 1 ? 1 : prm->num_thread;
   em_match_kernel<<<div_up((int)total, EM_WARPS), EM_WARPS * 32, 0, c->stream>>>(c->dc, a);

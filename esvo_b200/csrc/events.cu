@@ -158,7 +158,6 @@ __global__ void ew_lower_bounds_kernel(const int64_t* __restrict__ et, const int
 }
 
 // --------------------------------------------------------------------------------------------
-template <class T> static cudaError_t dmalloc(T** p, size_t n) { return cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)); }
 
 static int ew_alloc(Ctx* c, size_t cap) {
   Ctx::EventWindow& w = c->evw;

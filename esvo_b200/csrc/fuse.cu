@@ -61,8 +61,6 @@ struct MapState {
   unsigned long long* h_scal = nullptr;
 };
 
-template <class T> static cudaError_t dm(T** p, size_t n) { return cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)); }
-
 __device__ __forceinline__ void cam2world_f(const DevConsts& dc, double x, double y, double rho, double& p0, double& p1, double& p2) {
   const double z = 1.0 / rho;
   p0 = (x - dc.cx - dc.Pl[3] / z) * z / dc.fx;
@@ -809,7 +807,7 @@ __global__ void __launch_bounds__(1024) sgm_points_kernel(DevConsts dc, const in
 // T_world_cam = pose of the current map (host copy kept by fuse_reset_map), passed by value
 int sgm_points(Ctx* c, const int16_t* d_disp, const uint16_t* d_ex, const uint16_t* d_ey, size_t n, esvo_depth_point* out,
                unsigned long long* out_cnt) {
-  Pose16 Twc; std::memcpy(Twc.m, c->map->T_world_frame, 128);
+  Pose16 Twc; std::memcpy(Twc.m, c->slot().map->T_world_frame, 128);
   sgm_points_kernel<<<1, 1024, 0, c->stream>>>(c->dc, d_disp, d_ex, d_ey, (int)n, c->d_lut, Twc, c->prm.invdepth_min_range,
                                                c->prm.invdepth_max_range, (long long)c->prm.age_vis_threshold, out, out_cnt);
   c->launches += 1;
@@ -823,8 +821,7 @@ __global__ void fill_i32_kernel(int32_t* p, size_t n, int32_t v) {
 }
 
 // --------------------------------------------------------------------------------------------
-static int prop_reserve(Ctx* c, size_t need) {
-  MapState* ms = c->map;
+static int prop_reserve(Ctx* c, MapState* ms, size_t need) {
   if (need <= ms->prop_cap) return ESVO_OK;
   if (ms->staged) { c->set_error("internal: staging buffer grown while points are staged"); return ESVO_ERR_STATE; }
   size_t cap = std::max<size_t>(need, 65536);
@@ -832,44 +829,43 @@ static int prop_reserve(Ctx* c, size_t need) {
   void* olds[] = {P.hot, P.ok, P.rho, P.s2, P.nu, P.var, P.res, P.x0, P.x1, P.pc0, P.pc1, P.pc2, P.age, P.row, P.col, ms->next,
                   ms->cbits, ms->cprefix, ms->sort_pool};
   for (void* p : olds) if (p) cudaFree(p);
-  ESVO_CUDA_TRY(c, dm(&P.ok, cap)); ESVO_CUDA_TRY(c, dm(&P.hot, cap));
+  ESVO_CUDA_TRY(c, dmalloc(&P.ok, cap)); ESVO_CUDA_TRY(c, dmalloc(&P.hot, cap));
   double** ds[] = {&P.rho, &P.s2, &P.nu, &P.var, &P.res, &P.x0, &P.x1, &P.pc0, &P.pc1, &P.pc2};
-  for (double** d : ds) ESVO_CUDA_TRY(c, dm(d, cap));
-  ESVO_CUDA_TRY(c, dm(&P.age, cap)); ESVO_CUDA_TRY(c, dm(&P.row, cap)); ESVO_CUDA_TRY(c, dm(&P.col, cap));
-  ESVO_CUDA_TRY(c, dm(&ms->next, cap * 9)); ESVO_CUDA_TRY(c, dm(&ms->sort_pool, cap * 9));
+  for (double** d : ds) ESVO_CUDA_TRY(c, dmalloc(d, cap));
+  ESVO_CUDA_TRY(c, dmalloc(&P.age, cap)); ESVO_CUDA_TRY(c, dmalloc(&P.row, cap)); ESVO_CUDA_TRY(c, dmalloc(&P.col, cap));
+  ESVO_CUDA_TRY(c, dmalloc(&ms->next, cap * 9)); ESVO_CUDA_TRY(c, dmalloc(&ms->sort_pool, cap * 9));
   ms->cbits_words = (cap * 9 + 31) / 32;
-  ESVO_CUDA_TRY(c, dm(&ms->cbits, ms->cbits_words)); ESVO_CUDA_TRY(c, dm(&ms->cprefix, ms->cbits_words));
+  ESVO_CUDA_TRY(c, dmalloc(&ms->cbits, ms->cbits_words)); ESVO_CUDA_TRY(c, dmalloc(&ms->cprefix, ms->cbits_words));
   ms->prop_cap = cap;
   return ESVO_OK;
 }
 
-int fuse_alloc(Ctx* c) {
+int fuse_alloc(Ctx* c, MapState** out) {
   MapState* ms = new MapState();
-  c->map = ms;
+  *out = ms;
   const size_t npix = (size_t)c->dc.W * c->dc.H;
   MapSoA& M = ms->m;
   std::memset(&M, 0, sizeof(M)); std::memset(&ms->p, 0, sizeof(ms->p));
-  ESVO_CUDA_TRY(c, dm(&M.exists, npix));
+  ESVO_CUDA_TRY(c, dmalloc(&M.exists, npix));
   double** ds[] = {&M.rho, &M.s2, &M.nu, &M.var, &M.res, &M.x0, &M.x1, &M.pc0, &M.pc1, &M.pc2, &M.rho_tmp};
-  for (double** d : ds) ESVO_CUDA_TRY(c, dm(d, npix));
-  ESVO_CUDA_TRY(c, dm(&M.age, npix)); ESVO_CUDA_TRY(c, dm(&M.row, npix)); ESVO_CUDA_TRY(c, dm(&M.col, npix));
-  ESVO_CUDA_TRY(c, dm(&M.first_key, npix));
-  ESVO_CUDA_TRY(c, dm(&ms->head, npix));
-  ESVO_CUDA_TRY(c, dm(&ms->active, npix));
-  ESVO_CUDA_TRY(c, dm(&ms->pcnt, npix)); ESVO_CUDA_TRY(c, dm(&ms->active_sorted, npix));
+  for (double** d : ds) ESVO_CUDA_TRY(c, dmalloc(d, npix));
+  ESVO_CUDA_TRY(c, dmalloc(&M.age, npix)); ESVO_CUDA_TRY(c, dmalloc(&M.row, npix)); ESVO_CUDA_TRY(c, dmalloc(&M.col, npix));
+  ESVO_CUDA_TRY(c, dmalloc(&M.first_key, npix));
+  ESVO_CUDA_TRY(c, dmalloc(&ms->head, npix));
+  ESVO_CUDA_TRY(c, dmalloc(&ms->active, npix));
+  ESVO_CUDA_TRY(c, dmalloc(&ms->pcnt, npix)); ESVO_CUDA_TRY(c, dmalloc(&ms->active_sorted, npix));
   ESVO_CUDA_TRY(c, cudaMemset(ms->pcnt, 0, npix * 4));       // invariant: every fold zeroes the counts it consumed
-  ESVO_CUDA_TRY(c, dm(&ms->d_dl, npix)); ESVO_CUDA_TRY(c, dm(&ms->d_dl_keys, npix));
-  ESVO_CUDA_TRY(c, dm(&ms->d_scal, 8));
+  ESVO_CUDA_TRY(c, dmalloc(&ms->d_dl, npix)); ESVO_CUDA_TRY(c, dmalloc(&ms->d_dl_keys, npix));
+  ESVO_CUDA_TRY(c, dmalloc(&ms->d_scal, 8));
   ESVO_CUDA_TRY(c, cudaMallocHost((void**)&ms->h_scal, 4 * 8));
   ESVO_CUDA_TRY(c, cudaMemset(M.exists, 0, npix));
   ESVO_CUDA_TRY(c, cudaMemset(ms->head, 0xff, npix * 4));   // invariant: every fold leaves the heads it consumed at -1
   ESVO_CUDA_TRY(c, cudaMemset(ms->d_scal, 0, 8 * 8));
   for (int i = 0; i < 16; ++i) ms->T_world_frame[i] = ms->T_frame_world[i] = (i % 5 == 0) ? 1.0 : 0.0;
   ms->list_valid = true; ms->folds = 0;
-  return prop_reserve(c, 65536);
+  return prop_reserve(c, ms, 65536);
 }
-void fuse_free(Ctx* c) {
-  MapState* ms = c->map;
+void fuse_free(MapState* ms) {
   if (!ms) return;
   MapSoA& M = ms->m; PropSoA& P = ms->p;
   void* ps[] = {M.exists, M.rho, M.s2, M.nu, M.var, M.res, M.x0, M.x1, M.pc0, M.pc1, M.pc2, M.rho_tmp, M.age, M.row, M.col,
@@ -878,23 +874,17 @@ void fuse_free(Ctx* c) {
   for (void* p : ps) if (p) cudaFree(p);
   if (ms->h_scal) cudaFreeHost(ms->h_scal);
   delete ms;
-  c->map = nullptr;
 }
 
 // New empty DepthFrame at pose T (esvo_Mapping.cpp:268-272).  Two enqueued operations: clear the existence plane and the
 // map scalars {n_fusions, download count, map size, active pixels}.  The frame pose travels to the kernels by value.
 int fuse_reset_map(Ctx* c, const double T[16]) {
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   const size_t npix = (size_t)c->dc.W * c->dc.H;
   ESVO_CUDA_TRY(c, cudaMemsetAsync(ms->m.exists, 0, npix, c->stream));
   ESVO_CUDA_TRY(c, cudaMemsetAsync(ms->d_scal, 0, 64, c->stream));
   std::memcpy(ms->T_world_frame, T, 128);
-  // rigid inverse (kindr Transformation::inverse)
-  double* I = ms->T_frame_world;
-  for (int i = 0; i < 16; ++i) I[i] = 0;
-  I[15] = 1;
-  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) I[i * 4 + j] = T[j * 4 + i];
-  for (int i = 0; i < 3; ++i) { double s = 0; for (int k = 0; k < 3; ++k) s += I[i * 4 + k] * T[k * 4 + 3]; I[i * 4 + 3] = -s; }
+  rigid_inverse(T, ms->T_frame_world);
   ms->seq_base = 0; ms->staged = 0;
   ms->list_valid = true; ms->folds = 0; ms->cleaned = false;
   return ESVO_OK;
@@ -903,7 +893,7 @@ int fuse_reset_map(Ctx* c, const double T[16]) {
 // First staging call of a round that does not follow a reset: restart the active list (it then covers this round's pixels
 // only, which is all the fold needs; kernels that need EVERY existing pixel fall back to their full-image form).
 static int fuse_begin_round(Ctx* c) {
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   if (ms->staged == 0 && ms->folds > 0) {
     ESVO_CUDA_TRY(c, cudaMemsetAsync(ms->d_scal + 3, 0, 24, c->stream));   // active count, (spare), sort-pool cursor
     ms->list_valid = false;
@@ -914,11 +904,11 @@ static int fuse_begin_round(Ctx* c) {
 // Stage one vector of DepthPoints (device array).  n_cap bounds the count when it lives on the device.
 // naive != 0: naive_propagate_one_point (:290-327) -- the Gaussian propagation whatever LSnorm is.
 int fuse_points(Ctx* c, const esvo_depth_point* d_pts, size_t n_cap, const uint64_t* d_n, int radius, int naive) {
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   if (n_cap == 0) return ESVO_OK;
   if (ms->staged + n_cap > ms->prop_cap) {
     if (ms->staged) { c->set_error("fusion staging capacity exceeded"); return ESVO_ERR_CAPACITY; }
-    int rc = prop_reserve(c, n_cap);
+    int rc = prop_reserve(c, ms, n_cap);
     if (rc) return rc;
   }
   int rc = fuse_begin_round(c);
@@ -939,7 +929,7 @@ int fuse_points(Ctx* c, const esvo_depth_point* d_pts, size_t n_cap, const uint6
 
 // Stage a whole window (vectors given newest first) with as few launches as possible.
 int fuse_window(Ctx* c, const Ctx::WinFrame* frames, int nframes, int radius) {
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   const int B = 64;
   int rc = fuse_begin_round(c);
   if (rc) return rc;
@@ -967,7 +957,7 @@ int fuse_window(Ctx* c, const Ctx::WinFrame* frames, int nframes, int radius) {
 // Ordered per-pixel replay of everything staged since the last fold.  clean_* != null: SmartGrid::clean applied to the
 // folded pixels on the way out (whole-frame path: the map was reset, so the folded pixels are all there is).
 int fuse_finish(Ctx* c, bool naive, const double* clean4) {
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   if (ms->staged == 0) return ESVO_OK;
   CleanArgs ca{0, 0, 0, 0, 0};
   if (clean4) { ca.enable = 1; ca.var_thr = clean4[0]; ca.age_thr = clean4[1]; ca.rmax = clean4[2]; ca.rmin = clean4[3]; }
@@ -999,15 +989,16 @@ static bool list_ok(const MapState* ms) { return ms->list_valid && ms->folds == 
 
 int map_clean(Ctx* c, double var_thr, double age_thr, double rmax, double rmin) {
   const int npix = c->dc.W * c->dc.H, B = 256;
-  map_clean_kernel<<<div_up(npix, B), B, 0, c->stream>>>(npix, c->map->m, var_thr, age_thr, rmax, rmin);
+  MapState* ms = c->slot().map;
+  map_clean_kernel<<<div_up(npix, B), B, 0, c->stream>>>(npix, ms->m, var_thr, age_thr, rmax, rmin);
   c->launches += 1;
-  c->map->cleaned = true;
+  ms->cleaned = true;
   return ESVO_OK;
 }
 
 // DepthRegularization::apply; count != 0 also leaves the number of map elements in d_scal[2] (zeroed by the reset).
 int map_regularize(Ctx* c, bool count) {
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   const int npix = c->dc.W * c->dc.H, B = 32;
   if (list_ok(ms)) {
     // persistent: one-warp blocks walk the active list, one warp per pixel.  One-warp blocks (4 K registers) slot into the
@@ -1033,12 +1024,12 @@ int map_regularize(Ctx* c, bool count) {
 // h_counters (pinned, optional): receives a copy of the frame's kCounters device counters.
 int map_gather_async(Ctx* c, esvo_depth_point* d_out, unsigned long long* d_keys, unsigned long long* d_scal4,
                      unsigned long long* h_scal8, esvo_depth_point* h_sorted, uint64_t* h_counters) {
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   const int npix = c->dc.W * c->dc.H, B = 128;
   Pose16 Twf; std::memcpy(Twf.m, ms->T_world_frame, 128);
   if (h_sorted && list_ok(ms) && ms->fold_words && !ms->cleaned) {
     // sort-free: rank from the creator bitmap; the kernels write elements, scalars and counters straight into pinned memory
-    map_cbits_prefix_kernel<<<1, 1024, 0, c->stream>>>(ms->cbits, ms->cprefix, (int)ms->fold_words, ms->d_scal, h_scal8, c->d_counters, h_counters);
+    map_cbits_prefix_kernel<<<1, 1024, 0, c->stream>>>(ms->cbits, ms->cprefix, (int)ms->fold_words, ms->d_scal, h_scal8, c->slot().d_counters, h_counters);
     map_gather_list_kernel<<<div_up(npix, B), B, 0, c->stream>>>(ms->m, Twf, ms->active, ms->d_scal, ms->cbits, ms->cprefix, h_sorted);
     c->launches += 2;
     ESVO_CUDA_TRY(c, cudaGetLastError());
@@ -1053,7 +1044,7 @@ int map_gather_async(Ctx* c, esvo_depth_point* d_out, unsigned long long* d_keys
   }
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(h_scal8, d_scal4, 32, cudaMemcpyDeviceToHost, c->stream));
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(h_scal8 + 4, ms->d_scal, 32, cudaMemcpyDeviceToHost, c->stream));
-  if (h_counters) ESVO_CUDA_TRY(c, cudaMemcpyAsync(h_counters, c->d_counters, kCounters * 8, cudaMemcpyDeviceToHost, c->stream));
+  if (h_counters) ESVO_CUDA_TRY(c, cudaMemcpyAsync(h_counters, c->slot().d_counters, kCounters * 8, cudaMemcpyDeviceToHost, c->stream));
   ESVO_CUDA_TRY(c, cudaGetLastError());
   return ESVO_OK;
 }
@@ -1080,10 +1071,10 @@ int map_publish(Ctx* c, const double T[16], size_t* n) {
   Ctx::Published& pb = c->pub;
   const size_t npix = (size_t)c->dc.W * c->dc.H;
   if (!pb.xyz) {
-    ESVO_CUDA_TRY(c, dm(&pb.xyz, 3 * npix)); ESVO_CUDA_TRY(c, dm(&pb.sorted, npix)); ESVO_CUDA_TRY(c, dm(&pb.d_scal, 4));
+    ESVO_CUDA_TRY(c, dmalloc(&pb.xyz, 3 * npix)); ESVO_CUDA_TRY(c, dmalloc(&pb.sorted, npix)); ESVO_CUDA_TRY(c, dmalloc(&pb.d_scal, 4));
     ESVO_CUDA_TRY(c, cudaMallocHost((void**)&pb.h_scal, 8 * 8));
   }
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   int rc = map_gather_async(c, ms->d_dl, ms->d_dl_keys, pb.d_scal, pb.h_scal, pb.sorted, nullptr);
   if (rc) return rc;
   ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
@@ -1099,7 +1090,7 @@ int map_publish(Ctx* c, const double T[16], size_t* n) {
 }
 
 int map_download(Ctx* c, esvo_depth_point* out, size_t* n) {
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   const int npix = c->dc.W * c->dc.H, B = 128;
   Pose16 Twf; std::memcpy(Twf.m, ms->T_world_frame, 128);
   ESVO_CUDA_TRY(c, cudaMemsetAsync(ms->d_scal + 1, 0, 8, c->stream));
@@ -1132,7 +1123,7 @@ __global__ void map_count_kernel(int npix, MapSoA M, unsigned long long* scal) {
 }
 // counts existing map pixels into scal[2]
 int map_count(Ctx* c) {
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   if (list_ok(ms)) {   // scal[2] is still zero from the reset
     map_commit_count_list_kernel<<<div_up(c->dc.W * c->dc.H, 256), 256, 0, c->stream>>>(ms->m, 0, ms->active, ms->d_scal);
     c->launches += 1;
@@ -1145,20 +1136,17 @@ int map_count(Ctx* c) {
   return ESVO_OK;
 }
 int fuse_zero_fusion_counter(Ctx* c) {
-  ESVO_CUDA_TRY(c, cudaMemsetAsync(c->map->d_scal, 0, 8, c->stream));
+  ESVO_CUDA_TRY(c, cudaMemsetAsync(c->slot().map->d_scal, 0, 8, c->stream));
   return ESVO_OK;
 }
 // D2H of the map scalars: out[0] = n_fusions since the last zeroing, out[2] = map size (after map_count)
 int fuse_fetch_scalars(Ctx* c, unsigned long long out[4]) {
-  MapState* ms = c->map;
+  MapState* ms = c->slot().map;
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(ms->h_scal, ms->d_scal, 32, cudaMemcpyDeviceToHost, c->stream));
   ESVO_CUDA_TRY(c, cudaStreamSynchronize(c->stream));
   for (int i = 0; i < 4; ++i) out[i] = ms->h_scal[i];
   return ESVO_OK;
 }
-int fuse_reserve(Ctx* c, size_t total_points) { return prop_reserve(c, total_points); }
-const double* fuse_frame_pose(Ctx* c) { return c->map->T_world_frame; }
-// a kernel outside fuse.cu (or an API call that edits the map image-wide) invalidates the "all existing pixels are listed" property
-void fuse_list_invalidate(Ctx* c) { c->map->list_valid = false; }
+int fuse_reserve(Ctx* c, size_t total_points) { return prop_reserve(c, c->slot().map, total_points); }
 
 }  // namespace esvo

@@ -926,11 +926,12 @@ __global__ void __launch_bounds__(1024) cull_points_kernel(esvo_depth_point* pts
 }
 
 int lm_run(Ctx* c, const esvo_seed* d_seeds, size_t n_fixed) {
+  const SlotBufs& f = c->slot();
   LmArgs a;
-  a.seeds = d_seeds; a.n_ptr = n_fixed ? nullptr : (const unsigned long long*)(c->d_counters + 1);
-  a.n_fixed = (int)n_fixed; a.tl = c->obs_ls; a.tr = c->obs_rs; std::memcpy(a.T_left_world, c->T_left_world_inv, sizeof(a.T_left_world));
-  a.flag = c->lm_flag; a.res = c->lm_res; a.counters = (unsigned long long*)c->d_counters;
-  const int upper = (int)(n_fixed ? n_fixed : c->n_ev);
+  a.seeds = d_seeds; a.n_ptr = n_fixed ? nullptr : (const unsigned long long*)(f.d_counters + 1);
+  a.n_fixed = (int)n_fixed; a.tl = f.obs_ls; a.tr = f.obs_rs; std::memcpy(a.T_left_world, f.T_left_world_inv, sizeof(a.T_left_world));
+  a.flag = f.lm_flag; a.res = f.lm_res; a.counters = (unsigned long long*)f.d_counters;
+  const int upper = (int)(n_fixed ? n_fixed : f.n_ev);
   if (upper == 0) return ESVO_OK;
   // Tdist with up to 7 slots per lane: lm2_kernel at 20 seeds per SM.  On an H100 SXM (700 W limit, bench.py --no-parity
   // --no-extras --no-cpu-baseline) 20 beat 16 / 24 / 32 seeds per SM both as an isolated launch (0.62 vs 0.64 / 0.73 /
@@ -945,26 +946,25 @@ int lm_run(Ctx* c, const esvo_seed* d_seeds, size_t n_fixed) {
   return ESVO_OK;
 }
 
-// cull != 0: fuse pointCulling; the seeds are c->d_seeds unless given.
+// cull != 0: fuse pointCulling; out == null: the slot's d_pts.
 int points_order_impl(Ctx* c, const esvo_seed* d_seeds, size_t n_fixed, int cull, double std_thr, double cost_thr,
                       double rmin, double rmax, esvo_depth_point* out, unsigned long long* out_cnt) {
+  const SlotBufs& f = c->slot();
   CullArgs ca{cull, std_thr * std_thr, cost_thr, rmin, rmax};
   // the seed count lives on the device in the whole-frame path: the grid covers the event capacity, surplus blocks exit
-  const int upper = (int)(n_fixed ? n_fixed : c->n_ev);
+  const int upper = (int)(n_fixed ? n_fixed : f.n_ev);
   points_order_kernel<<<std::max(1, div_up(upper, kOrdBlockP)), kOrdBlockP, 0, c->stream>>>(
-      c->dc, d_seeds, n_fixed ? nullptr : (const unsigned long long*)(c->d_counters + 1), (int)n_fixed, c->lm_flag, c->lm_res, ca,
-      out ? out : c->d_pts, out_cnt, (unsigned long long*)c->d_counters);
+      c->dc, d_seeds, n_fixed ? nullptr : (const unsigned long long*)(f.d_counters + 1), (int)n_fixed, f.lm_flag, f.lm_res, ca,
+      out ? out : f.d_pts, out_cnt, (unsigned long long*)f.d_counters);
   c->launches += 1;
   ESVO_CUDA_TRY(c, cudaGetLastError());
   return ESVO_OK;
 }
-int points_order(Ctx* c, int cull, double std_thr, double cost_thr, double rmin, double rmax) {
-  return points_order_impl(c, c->d_seeds, 0, cull, std_thr, cost_thr, rmin, rmax, nullptr, nullptr);
-}
-// in: d_pts[0..n) (device), out: c->d_pts, count in counters[3]
+// in: d_pts[0..n) (device), out: the slot's d_pts, count in counters[3]
 int cull_points(Ctx* c, esvo_depth_point* d_in, size_t n, double std_thr, double cost_thr, double rmin, double rmax) {
+  const SlotBufs& f = c->slot();
   CullArgs ca{1, std_thr * std_thr, cost_thr, rmin, rmax};
-  cull_points_kernel<<<1, kOrderThreads, 0, c->stream>>>(d_in, (int)n, ca, c->d_pts, (unsigned long long*)c->d_counters);
+  cull_points_kernel<<<1, kOrderThreads, 0, c->stream>>>(d_in, (int)n, ca, f.d_pts, (unsigned long long*)f.d_counters);
   c->launches += 1;
   ESVO_CUDA_TRY(c, cudaGetLastError());
   return ESVO_OK;

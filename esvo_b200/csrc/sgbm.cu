@@ -67,8 +67,6 @@ __global__ void sgbm_median_kernel(const int16_t* raw, Dims dm, int16_t* out) {
   out[t] = median3(raw, dm, y, x);
 }
 
-template <class T> static cudaError_t dmalloc(T** p, size_t n) { return cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)); }
-
 // d_left / d_right: device images with row pitch `pitch`; d_out: H*W int16 on the device.
 int sgbm_run(Ctx* c, const uint8_t* d_left, const uint8_t* d_right, int pitch, const Dims& dm, int16_t* d_out) {
   const size_t vol = (size_t)dm.H * dm.W1 * dm.D, rows = (size_t)dm.H * 6 * dm.W;

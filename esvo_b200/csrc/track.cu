@@ -60,8 +60,6 @@ struct TrackState {
   int rand_() { uint32_t n = hist[pos] + hist[(pos + 28) % 31]; hist[pos] = n; pos = (pos + 1) % 31; return (int)(n >> 1); }
 };
 
-template <class T> static cudaError_t dm(T** p, size_t n) { return cudaMalloc((void**)p, std::max<size_t>(n, 1) * sizeof(T)); }
-
 // ---- negative TS: 255 - GaussianBlur5x5(u8) (kernelSize 5) or 255 - TS (kernelSize 0) ----
 __device__ __forceinline__ int refl101t(int p, int len) {
   if (len == 1) return 0;
@@ -706,12 +704,12 @@ int track_alloc(Ctx* c) {
   t->srand_(1);
   const size_t npix = (size_t)c->dc.W * c->dc.H, nimg = (size_t)c->dc.pitch * c->dc.H;
   TrkDev& d = t->d;
-  ESVO_CUDA_TRY(c, dm(&d.ts, nimg)); ESVO_CUDA_TRY(c, dm(&d.neg, nimg));
-  ESVO_CUDA_TRY(c, dm(&d.du, npix)); ESVO_CUDA_TRY(c, dm(&d.dv, npix));
-  ESVO_CUDA_TRY(c, dm(&d.state, 64));
+  ESVO_CUDA_TRY(c, dmalloc(&d.ts, nimg)); ESVO_CUDA_TRY(c, dmalloc(&d.neg, nimg));
+  ESVO_CUDA_TRY(c, dmalloc(&d.du, npix)); ESVO_CUDA_TRY(c, dmalloc(&d.dv, npix));
+  ESVO_CUDA_TRY(c, dmalloc(&d.state, 64));
   ESVO_CUDA_TRY(c, cudaMemset(d.ts, 0, nimg));
   d.cap = 4096;
-  ESVO_CUDA_TRY(c, dm(&d.xyz, d.cap * 3)); ESVO_CUDA_TRY(c, dm(&d.items, d.cap * 3));
+  ESVO_CUDA_TRY(c, dmalloc(&d.xyz, d.cap * 3)); ESVO_CUDA_TRY(c, dmalloc(&d.items, d.cap * 3));
   static bool attr_set = false;
   (void)attr_set;
   const int smem = (TRK_MAXB * 6 + TRK_MAXB * 2 + TRK_MAXB * 3 + 16 * 8) * 8;
@@ -743,12 +741,10 @@ static bool inverse4_host(const double* A, double* inv) {
   return true;
 }
 
-#define CHECK_CTX(c) do { if (!(c)) return ESVO_ERR_INVALID_ARG; cudaSetDevice((c)->device); } while (0)
-
 // resetRegProblem / setProblem for both forms: ref_xyz != NULL is the caller's host cloud of n points, shuffled in place;
 // ref_xyz == NULL is the adopted device cloud, shuffled through TrackState::perm.  Same rand() draws in the same order.
 static int track_reset(esvo_ctx* c, float* ref_xyz, size_t n, const double Twr[16], const double Twc[16], const uint8_t* ts_left) {
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   const esvo_params& p = c->prm;
   if (p.trk_patch_size_x != 1 || p.trk_patch_size_y != 1) { c->set_error("tracking patch must be 1x1 (as in every shipped cfg)"); return ESVO_ERR_UNSUPPORTED; }
   if (p.trk_batch_size > TRK_MAXB || p.trk_batch_size < 6) { c->set_error("BATCH_SIZE must be in [6,1024]"); return ESVO_ERR_UNSUPPORTED; }
@@ -781,11 +777,11 @@ static int track_reset(esvo_ctx* c, float* ref_xyz, size_t n, const double Twr[1
   if (numPoints > d.cap) {
     cudaFree(d.xyz); cudaFree(d.items);
     d.cap = numPoints;
-    ESVO_CUDA_TRY(c, dm(&d.xyz, d.cap * 3)); ESVO_CUDA_TRY(c, dm(&d.items, d.cap * 3));
+    ESVO_CUDA_TRY(c, dmalloc(&d.xyz, d.cap * 3)); ESVO_CUDA_TRY(c, dmalloc(&d.items, d.cap * 3));
   }
   if (ref_xyz) ESVO_CUDA_TRY(c, cudaMemcpyAsync(d.xyz, ref_xyz, numPoints * 3 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
   else {   // only the sampled indices travel; the cloud itself is never moved
-    if (numPoints > d.idx_cap) { cudaFree(d.idx); d.idx_cap = numPoints; ESVO_CUDA_TRY(c, dm(&d.idx, d.idx_cap)); }
+    if (numPoints > d.idx_cap) { cudaFree(d.idx); d.idx_cap = numPoints; ESVO_CUDA_TRY(c, dmalloc(&d.idx, d.idx_cap)); }
     ESVO_CUDA_TRY(c, cudaMemcpyAsync(d.idx, t->perm.data(), numPoints * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   }
   ESVO_CUDA_TRY(c, cudaMemcpyAsync(d.state, state, sizeof(state), cudaMemcpyHostToDevice, c->stream));
@@ -820,7 +816,7 @@ ESVO_API int esvo_track_reset(esvo_ctx* c, float* ref_xyz, size_t n, const doubl
 
 ESVO_API int esvo_track_adopt_map_dev(esvo_ctx* c, int64_t stamp, size_t* n_points) {
   CHECK_CTX(c);
-  if (c->depth > 1) { int rc0 = drain(c); if (rc0) return rc0; }
+  if (int rc0 = drain_if_pipelined(c)) return rc0;
   const Ctx::Published& pb = c->pub;
   if (!pb.valid || pb.stamp != stamp) {
     c->set_error("esvo_track_adopt_map_dev: the newest cloud published on this context is not the one of stamp " + std::to_string((long long)stamp));
@@ -828,7 +824,7 @@ ESVO_API int esvo_track_adopt_map_dev(esvo_ctx* c, int64_t stamp, size_t* n_poin
   }
   TrackState* t = c->trk;
   TrkDev& d = t->d;
-  if (pb.n > d.ref_cap) { cudaFree(d.ref); d.ref_cap = pb.n; ESVO_CUDA_TRY(c, dm(&d.ref, 3 * d.ref_cap)); }
+  if (pb.n > d.ref_cap) { cudaFree(d.ref); d.ref_cap = pb.n; ESVO_CUDA_TRY(c, dmalloc(&d.ref, 3 * d.ref_cap)); }
   // a snapshot: the mapper may publish again before the next tracking pass
   if (pb.n) ESVO_CUDA_TRY(c, cudaMemcpyAsync(d.ref, pb.xyz, pb.n * 3 * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
   t->perm.resize(pb.n);

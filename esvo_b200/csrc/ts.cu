@@ -411,7 +411,6 @@ __global__ void fill_i64_kernel(long long* p, size_t n, long long v) {
 }
 
 // --------------------------------------------------------------------------------------------
-template <class T> static cudaError_t dmalloc(T** p, size_t n) { return cudaMalloc((void**)p, n * sizeof(T)); }
 
 int ts_reset_state(Ctx* c, int cam) {
   TsState& s = c->ts[cam];

@@ -119,16 +119,22 @@ def test_full_size_frame_properties(product_lib, rig, n_seeds):
 
 
 def test_pipeline_depth_invariance_full_size(product_lib):
-    """Frames processed with 1, 3 and 8 frames in flight give byte-identical maps and counters."""
+    """Frames processed with 1, 3 and 8 frames in flight give byte-identical maps and counters, and so does one context
+    whose depth changes between frames (3, 3, 1, 4: every outstanding ticket is collected before each switch)."""
     s = [synth.make_stream("hkust", seed=4, n_seeds=5000, t_ts=t, history_ms=50.0) for t in (0.50, 0.55, 0.60, 0.65)]
     ref = None
-    for depth in (1, 3, 8):
+    for schedule in ((1,) * 4, (3,) * 4, (8,) * 4, (3, 3, 1, 4)):
         def tw(p):
             p.max_num_fusion_frames = 3
         g = _gpu_backend(product_lib, "hkust", tweak=tw)
-        g.set_pipeline_depth(depth)
         tickets, got = [], []
-        for f in s:
+        depth = None
+        for f, d in zip(s, schedule):
+            if d != depth:
+                while tickets:
+                    m, c = g.results_end(tickets.pop(0)); got.append((c, m.tobytes()))
+                depth = d
+                g.set_pipeline_depth(depth)
             if len(tickets) >= max(1, depth - 1):
                 m, c = g.results_end(tickets.pop(0)); got.append((c, m.tobytes()))
             for cam, side in ((0, "left"), (1, "right")):
@@ -147,7 +153,7 @@ def test_pipeline_depth_invariance_full_size(product_lib):
             ref = got
         else:
             assert [a[0] for a in got] == [a[0] for a in ref]
-            assert [a[1] for a in got] == [a[1] for a in ref], f"depth {depth} changed the maps"
+            assert [a[1] for a in got] == [a[1] for a in ref], f"depths {schedule} changed the maps"
 
 
 def test_mapping_tracking_loop_matches_oracle(oracle_lib, product_lib):
