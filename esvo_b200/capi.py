@@ -117,6 +117,16 @@ def _arr(a, dtype):
     return np.ascontiguousarray(a, dtype=dtype)
 
 
+def _wire_runs(runs):
+    """Byte buffers of whole wire records -> (the buffers as uint8 arrays, void* array, size_t record counts)."""
+    bufs = [np.frombuffer(r, np.uint8) if not isinstance(r, np.ndarray) else _arr(r, np.uint8).ravel() for r in runs]
+    for b in bufs:
+        assert b.size % EVENT_WIRE_DTYPE.itemsize == 0
+    ptrs = (C.c_void_p * max(1, len(bufs)))(*[b.ctypes.data if b.size else None for b in bufs])
+    ns = (C.c_size_t * max(1, len(bufs)))(*[b.size // EVENT_WIRE_DTYPE.itemsize for b in bufs])
+    return bufs, ptrs, ns
+
+
 @dataclass
 class Library:
     lib: C.CDLL
@@ -265,17 +275,45 @@ class Backend:
     def ts_push_event_array(self, cam, runs, ok=(0,)):
         """esvo_ts_push_event_array: runs is a list of byte buffers (bytes, bytearray, uint8 arrays), each a whole number of
         13-byte dvs_msgs/Event wire records (EVENT_WIRE_DTYPE).  Returns the return code (in ok, else EsvoError)."""
-        bufs = [np.frombuffer(r, np.uint8) if not isinstance(r, np.ndarray) else _arr(r, np.uint8).ravel() for r in runs]
-        for b in bufs:
-            assert b.size % EVENT_WIRE_DTYPE.itemsize == 0
-        ptrs = (C.c_void_p * max(1, len(bufs)))(*[b.ctypes.data if b.size else None for b in bufs])
-        ns = (C.c_size_t * max(1, len(bufs)))(*[b.size // EVENT_WIRE_DTYPE.itemsize for b in bufs])
+        bufs, ptrs, ns = _wire_runs(runs)
         return self._call("ts_push_event_array", [C.c_int, C.c_void_p, C.c_void_p, C.c_int], cam, C.cast(ptrs, C.c_void_p),
                           C.cast(ns, C.c_void_p), len(bufs), ok=ok)
 
     def ts_push_event_array_dev(self, cam, packed_dev_ptr, n, ok=(0,)):
         """esvo_ts_push_event_array_dev: n wire records at the device address packed_dev_ptr (an int, any alignment)."""
         return self._call("ts_push_event_array_dev", [C.c_int, C.c_void_p, C.c_size_t], cam, C.c_void_p(packed_dev_ptr), n, ok=ok)
+
+    def ts_events_pushed(self, cam):
+        """esvo_ts_events_pushed: events in the camera's log since create / ts_reset (with a hot-pixel mask, those kept)."""
+        total = C.c_int64(0)
+        self._call("ts_events_pushed", [C.c_int, C.POINTER(C.c_int64)], cam, C.byref(total))
+        return total.value
+
+    # ---- hot pixels (include/esvo_b200_hotpix.h) ----
+    def hotpix_count_event_array(self, cam, runs, ok=(0,)):
+        """esvo_hotpix_count_event_array: runs as for ts_push_event_array."""
+        bufs, ptrs, ns = _wire_runs(runs)
+        return self._call("hotpix_count_event_array", [C.c_int, C.c_void_p, C.c_void_p, C.c_int], cam, C.cast(ptrs, C.c_void_p),
+                          C.cast(ns, C.c_void_p), len(bufs), ok=ok)
+
+    def hotpix_count_event_array_dev(self, cam, packed_dev_ptr, n, ok=(0,)):
+        """esvo_hotpix_count_event_array_dev: n wire records at the device address packed_dev_ptr (an int, any alignment)."""
+        return self._call("hotpix_count_event_array_dev", [C.c_int, C.c_void_p, C.c_size_t], cam, C.c_void_p(packed_dev_ptr), n, ok=ok)
+
+    def hotpix_select(self, cam, k, ok=(0,)):
+        """esvo_hotpix_select -> (return code, number of hot pixels)."""
+        n_hot = C.c_int64(-1)
+        rc = self._call("hotpix_select", [C.c_int, C.c_double, C.POINTER(C.c_int64)], cam, float(k), C.byref(n_hot), ok=ok)
+        return rc, n_hot.value
+
+    def hotpix_read(self, cam):
+        """esvo_hotpix_read -> (counts H x W u32, mask H x W u8)."""
+        counts = np.empty(self.W * self.H, np.uint32); mask = np.empty(self.W * self.H, np.uint8)
+        self._call("hotpix_read", [C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_uint8)], cam, _ptr(counts, C.c_uint32), _ptr(mask, C.c_uint8))
+        return counts.reshape(self.H, self.W), mask.reshape(self.H, self.W)
+
+    def hotpix_clear(self, cam):
+        self._call("hotpix_clear", [C.c_int], cam)
 
     # ---- mapping ----
     def set_ts_pair(self, ts_left, ts_right, T_world_left):

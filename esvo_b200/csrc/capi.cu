@@ -422,6 +422,44 @@ ESVO_API int esvo_ts_push_event_array_dev(esvo_ctx* c, int cam, const uint8_t* p
   StreamScope sc(c, c->s_tsc[cam]);
   return ts_push_packed(c, cam, packed_dev, n, nullptr);
 }
+ESVO_API int esvo_ts_events_pushed(esvo_ctx* c, int cam, int64_t* total) {
+  CHECK_CTX(c);
+  if (cam < 0 || cam > 1 || !total) return ESVO_ERR_INVALID_ARG;
+  *total = c->ts[cam].log_base + (int64_t)c->ts[cam].log_n;
+  return ESVO_OK;
+}
+// ---------------- hot pixels (hotpix.cu) ----------------
+ESVO_API int esvo_hotpix_count_event_array(esvo_ctx* c, int cam, const uint8_t* const* runs, const size_t* n_events, int n_runs) {
+  CHECK_CTX(c);
+  if (cam < 0 || cam > 1 || n_runs < 0 || (n_runs && (!runs || !n_events))) return ESVO_ERR_INVALID_ARG;
+  for (int k = 0; k < n_runs; ++k) if (n_events[k] && !runs[k]) return ESVO_ERR_INVALID_ARG;
+  StreamScope sc(c, c->s_tsc[cam]);
+  return hp_count_packed_host(c, cam, runs, n_events, n_runs);
+}
+ESVO_API int esvo_hotpix_count_event_array_dev(esvo_ctx* c, int cam, const uint8_t* packed_dev, size_t n) {
+  CHECK_CTX(c);
+  if (cam < 0 || cam > 1 || (n && !packed_dev)) return ESVO_ERR_INVALID_ARG;
+  StreamScope sc(c, c->s_tsc[cam]);
+  return hp_count_packed(c, cam, packed_dev, n);
+}
+ESVO_API int esvo_hotpix_select(esvo_ctx* c, int cam, double k, int64_t* n_hot) {
+  CHECK_CTX(c);
+  if (cam < 0 || cam > 1) return ESVO_ERR_INVALID_ARG;
+  StreamScope sc(c, c->s_tsc[cam]);
+  return hp_select(c, cam, k, n_hot);
+}
+ESVO_API int esvo_hotpix_read(esvo_ctx* c, int cam, uint32_t* counts, uint8_t* mask) {
+  CHECK_CTX(c);
+  if (cam < 0 || cam > 1) return ESVO_ERR_INVALID_ARG;
+  StreamScope sc(c, c->s_tsc[cam]);
+  return hp_read(c, cam, counts, mask);
+}
+ESVO_API int esvo_hotpix_clear(esvo_ctx* c, int cam) {
+  CHECK_CTX(c);
+  if (cam < 0 || cam > 1) return ESVO_ERR_INVALID_ARG;
+  StreamScope sc(c, c->s_tsc[cam]);
+  return hp_clear(c, cam);
+}
 ESVO_API int esvo_run_ts_build(esvo_ctx* c, int cam, int64_t T) {
   CHECK_CTX(c);
   if (cam < 0 || cam > 1) return ESVO_ERR_INVALID_ARG;

@@ -49,18 +49,10 @@ __global__ void ts_ingest_kernel(const uint16_t* __restrict__ sx, const uint16_t
   if (x >= W || y >= H) return;
   atomicMax(&idx_grid[(size_t)y * W + x], gbase + (long long)i);
 }
-// ---- packed source: dvs_msgs/Event wire records, as a ROS bag's EventArray messages carry them.  Record i is 13 bytes at
-// src + 13 i, little-endian and unaligned: u16 x | u16 y | u32 sec | u32 nsec | u8 polarity.  Each warp stages the bytes of
-// its 32 records, and of the record before them (the order test), through shared memory with aligned 4-byte loads; only
-// the words at the two ends of the whole input are read byte by byte.  Then each lane decodes its record from shared memory.
+// ---- packed source: dvs_msgs/Event wire records (common.cuh).  Each warp stages its records through shared memory
+// (packed_stage_warp), then each lane decodes its record from there.
 // RAW = false: same writes, order flag and scatter as ts_ingest_kernel.  RAW = true: decode into the unordered path's
 // raw_* staging only (its run-max kernels do the rest).
-constexpr int kPackRec = 13, kPackWords = (kPackRec * 33 + 3 + 3) / 4;   // 32 records + the one before, any alignment
-__device__ __forceinline__ long long packed_stamp(const uint8_t* r) {   // ros::Time::toNSec(): sec * 1e9 + nsec, 64-bit
-  const unsigned sec = r[4] | (r[5] << 8) | (r[6] << 16) | ((unsigned)r[7] << 24);
-  const unsigned nsec = r[8] | (r[9] << 8) | (r[10] << 16) | ((unsigned)r[11] << 24);
-  return (long long)sec * 1000000000LL + (long long)nsec;
-}
 template <bool RAW>
 __global__ void __launch_bounds__(256) ts_ingest_packed_kernel(const uint8_t* __restrict__ src, size_t n,
                                                                uint16_t* __restrict__ ex, uint16_t* __restrict__ ey,
@@ -72,26 +64,9 @@ __global__ void __launch_bounds__(256) ts_ingest_packed_kernel(const uint8_t* __
   const size_t i0 = (blockIdx.x * (size_t)blockDim.x) + (size_t)w * 32;   // first record of this warp
   if (i0 >= n) return;
   const size_t i = i0 + lane;
-  const uintptr_t lo = (uintptr_t)src, hi = lo + n * kPackRec;           // the input's bytes [lo, hi)
-  const uintptr_t b0 = lo + (i0 > 0 ? i0 - 1 : 0) * kPackRec;            // the previous record's first byte (or the first one)
-  const uintptr_t b1 = lo + min(n, i0 + 32) * kPackRec;
-  const uintptr_t a0 = b0 & ~(uintptr_t)3;
-  const int nw = (int)((b1 - a0 + 3) >> 2);
-  for (int k = lane; k < nw; k += 32) {
-    const uintptr_t a = a0 + 4 * (uintptr_t)k;
-    uint32_t v;
-    if (a >= lo && a + 4 <= hi) v = *(const uint32_t*)a;
-    else {   // an end word of the input: only its bytes inside [lo, hi)
-      v = 0;
-      for (int q = 0; q < 4; ++q) if (a + q >= lo && a + q < hi) v |= (uint32_t)*(const uint8_t*)(a + q) << (8 * q);
-    }
-    stage[w][k] = v;
-  }
-  __syncwarp();
+  const uint8_t* r = packed_stage_warp(src, n, i0, lane, stage[w]);
   if (i >= n) return;
-  const uint8_t* sb = (const uint8_t*)stage[w];
-  const uint8_t* r = sb + (lo + i * kPackRec - a0);
-  const int x = r[0] | (r[1] << 8), y = r[2] | (r[3] << 8);
+  const int x = packed_x(r), y = packed_y(r);
   const long long t = packed_stamp(r);
   const uint8_t pol = r[12] != 0;   // the ROS bool
   ex[i] = (uint16_t)x; ey[i] = (uint16_t)y; et[i] = t; ep[i] = pol;
@@ -463,6 +438,7 @@ void ts_free(Ctx* c, int cam) {
   for (void* p : ps) if (p) cudaFree(p);
   if (s.h_pack) cudaFreeHost(s.h_pack);
   if (s.ev_pack) cudaEventDestroy(s.ev_pack);
+  hp_free(s);
   s = TsState();
 }
 
@@ -605,10 +581,21 @@ int ts_push(Ctx* c, int cam, const uint16_t* x, const uint16_t* y, const int64_t
 // n dvs_msgs/Event wire records (13 bytes each, any alignment) in device memory.  Everything after the decode is ts_push's:
 // the same log, push indices, order flag, fold and refusals.  host_last_t: the stamp of the last record when the host knows
 // it (the host form below), else null -- as for ts_push's host and device sources.
+// With a hot-pixel mask installed (esvo_hotpix_select) the records at hot pixels are dropped first (hp_compact_packed, one
+// read-back of the number kept and the last kept stamp) and the push continues on the kept records, with that stamp as
+// host_last_t.  The half-log refusal applies to the n records handed in, before the filter.
 int ts_push_packed(Ctx* c, int cam, const uint8_t* src, size_t n, const int64_t* host_last_t) {
   if (n == 0) return ESVO_OK;
   TsState& s = c->ts[cam];
-  int rc = ts_make_room(c, cam, n);
+  int rc;
+  int64_t kept_last_t;
+  if (s.hp.masked) {
+    if (n > s.log_cap / 2) { c->set_error("event batch larger than half the resident log"); return ESVO_ERR_CAPACITY; }
+    if ((rc = hp_compact_packed(c, cam, src, n, &src, &n, &kept_last_t))) return rc;
+    if (n == 0) return ESVO_OK;
+    host_last_t = &kept_last_t;
+  }
+  rc = ts_make_room(c, cam, n);
   if (rc) return rc;
   const size_t off = s.log_n;
   cudaEvent_t pe = c->prof_begin(0);
@@ -635,16 +622,10 @@ int ts_push_packed(Ctx* c, int cam, const uint8_t* src, size_t n, const int64_t*
   return ESVO_OK;
 }
 
-// Host runs of wire records (e.g. the event blocks of several EventArray messages in a memory-mapped bag): gathered with
-// memcpy into this camera's pinned staging block, one H2D copy, then ts_push_packed on the copy.  The staging block is
-// reused once the previous copy out of it has completed, so the caller's runs are free again on return.
-int ts_push_packed_host(Ctx* c, int cam, const uint8_t* const* runs, const size_t* n_events, int n_runs) {
+// The pinned staging block of camera cam and its device landing buffer, both at least `bytes` long, once the previous copy
+// out of the staging block has completed.
+int ts_pack_staging(Ctx* c, int cam, size_t bytes) {
   TsState& s = c->ts[cam];
-  size_t n = 0;
-  for (int k = 0; k < n_runs; ++k) n += n_events[k];
-  if (n == 0) return ESVO_OK;
-  if (n > s.log_cap / 2) { c->set_error("event batch larger than half the resident log"); return ESVO_ERR_CAPACITY; }
-  const size_t bytes = n * kPackRec;
   if (s.ev_pack) ESVO_CUDA_TRY(c, cudaEventSynchronize(s.ev_pack));
   else ESVO_CUDA_TRY(c, cudaEventCreateWithFlags(&s.ev_pack, cudaEventDisableTiming));
   if (bytes > s.h_pack_cap) {
@@ -660,6 +641,21 @@ int ts_push_packed_host(Ctx* c, int cam, const uint8_t* const* runs, const size_
     s.pack_cap = std::max<size_t>(2 * bytes, (size_t)1 << 20);
     ESVO_CUDA_TRY(c, dmalloc(&s.pack_dev, s.pack_cap));
   }
+  return ESVO_OK;
+}
+
+// Host runs of wire records (e.g. the event blocks of several EventArray messages in a memory-mapped bag): gathered with
+// memcpy into this camera's pinned staging block, one H2D copy, then ts_push_packed on the copy.  The staging block is
+// reused once the previous copy out of it has completed, so the caller's runs are free again on return.
+int ts_push_packed_host(Ctx* c, int cam, const uint8_t* const* runs, const size_t* n_events, int n_runs) {
+  TsState& s = c->ts[cam];
+  size_t n = 0;
+  for (int k = 0; k < n_runs; ++k) n += n_events[k];
+  if (n == 0) return ESVO_OK;
+  if (n > s.log_cap / 2) { c->set_error("event batch larger than half the resident log"); return ESVO_ERR_CAPACITY; }
+  const size_t bytes = n * kPackRec;
+  int rc = ts_pack_staging(c, cam, bytes);
+  if (rc) return rc;
   uint8_t* d = s.h_pack;
   for (int k = 0; k < n_runs; ++k) {
     if (!n_events[k]) continue;

@@ -5,15 +5,21 @@
 // trajectory and calls file of system_loop.cpp.
 // usage: bag_system <bag> <left events topic> <right events topic> <left camera_info topic> <right camera_info topic>
 //                   <result.bin> <trajectory.txt> [--t0-ns T] [--dt-ns D] [--ticks N] [--mapping-every M]
-//                   [--calls calls.txt] [--profile]
+//                   [--calls calls.txt] [--profile] [--hot-pixels K]
 //   --t0-ns: first sync tick (default: the first left event's stamp + dt); --dt-ns: tick period (default 10 ms, 100 Hz);
 //   --ticks: number of ticks (default: until every event of both topics has been delivered); --mapping-every: 5.
-// Exit codes: 0 done, 2 no CUDA device, 3 the bag cannot be read (the reason is printed), 64 usage.
+//   --hot-pixels K: before the first tick, count each events topic over the whole bag, select the hot pixels with k = K
+//   (include/esvo_b200_hotpix.h; 5 is the usual choice) and drop their events from then on, as the offline hot-pixel tool
+//   of the reference's data preparation does; prints the number of hot pixels per camera.
+// Exit codes: 0 done, 2 no CUDA device, 3 the bag cannot be read or its hot pixels cannot be selected (the reason is
+// printed), 64 usage.
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <vector>
 
 #include "esvo_b200/esvo_system.hpp"
 #include "esvo_b200/rosbag_events.hpp"
@@ -22,11 +28,12 @@
 int main(int argc, char** argv) {
   if (argc < 8) {
     std::printf("usage: bag_system <bag> <left events> <right events> <left camera_info> <right camera_info> <result.bin> "
-                "<trajectory.txt> [--t0-ns T] [--dt-ns D] [--ticks N] [--mapping-every M] [--calls calls.txt] [--profile]\n");
+                "<trajectory.txt> [--t0-ns T] [--dt-ns D] [--ticks N] [--mapping-every M] [--calls calls.txt] [--profile] [--hot-pixels K]\n");
     return 64;
   }
   int64_t t0 = INT64_MIN, dt = 10000000, n_ticks = -1;
   int mapping_every = 5;
+  double hot_k = -1;
   bool profile = false;
   const char* calls = nullptr;
   for (int i = 8; i < argc; ++i) {
@@ -38,6 +45,11 @@ int main(int argc, char** argv) {
     else if (a == "--mapping-every" && has) mapping_every = std::atoi(argv[++i]);
     else if (a == "--calls" && has) calls = argv[++i];
     else if (a == "--profile") profile = true;
+    else if (a == "--hot-pixels" && has) {
+      char* end = nullptr;
+      hot_k = std::strtod(argv[++i], &end);
+      if (*end || !(hot_k >= 0) || !std::isfinite(hot_k)) { std::printf("--hot-pixels takes a finite k >= 0\n"); return 64; }
+    }
     else { std::printf("unknown argument %s\n", a.c_str()); return 64; }
   }
   if (dt <= 0 || mapping_every <= 0) { std::printf("--dt-ns and --mapping-every must be positive\n"); return 64; }
@@ -58,6 +70,20 @@ int main(int argc, char** argv) {
   try { cs = std::make_shared<esvo::CameraSystem>(cal[0], cal[1], esvo_examples::hkustParams(), 0); }
   catch (const std::exception& e) { std::printf("%s\n", e.what()); return 2; }
   if (profile) esvo_profile(cs->ctx(), 0xff);
+  if (hot_k >= 0) {
+    for (int c = 0; c < 2; ++c) {
+      std::vector<const uint8_t*> ptr;
+      std::vector<size_t> n;
+      for (const esvo::EventRun& r : ev[c]->runs()) { ptr.push_back(r.data); n.push_back(r.n); }
+      int64_t n_hot = 0;
+      if (esvo_hotpix_count_event_array(cs->ctx(), c, ptr.data(), n.data(), (int)ptr.size()) != ESVO_OK ||
+          esvo_hotpix_select(cs->ctx(), c, hot_k, &n_hot) != ESVO_OK) {
+        std::printf("hot pixels: %s\n", esvo_last_error(cs->ctx()));
+        return 3;
+      }
+      std::printf("hot pixels %s: %lld\n", c ? "right" : "left", (long long)n_hot);
+    }
+  }
 
   esvo_core::esvo_System::Config cfg;
   cfg.t0_ns = t0; cfg.dt_ns = dt; cfg.mapping_every = mapping_every;

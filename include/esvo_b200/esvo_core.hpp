@@ -135,28 +135,28 @@ class TimeSurface {
   bool eventsCallback(const std::vector<esvo::Event>& events) {
     x_.resize(events.size()); y_.resize(events.size()); t_.resize(events.size()); p_.resize(events.size());
     for (size_t i = 0; i < events.size(); ++i) { x_[i] = events[i].x; y_[i] = events[i].y; t_[i] = events[i].ts; p_[i] = events[i].polarity; }
-    if (esvo_ts_push_events(cs_->ctx(), cam_, x_.data(), y_.data(), t_.data(), p_.data(), events.size()) != ESVO_OK) return false;
-    pushed_ += events.size();
-    return true;
+    return esvo_ts_push_events(cs_->ctx(), cam_, x_.data(), y_.data(), t_.data(), p_.data(), events.size()) == ESVO_OK;
   }
   // The same on packed runs of wire records (the events of one or more EventArray messages): copied as they are and
-  // decoded on the device (esvo_ts_push_event_array), no per-event host work.
+  // decoded on the device (esvo_ts_push_event_array), no per-event host work.  With a hot-pixel mask installed
+  // (esvo_hotpix_select) the events at hot pixels are dropped.
   bool eventsCallback(const std::vector<esvo::EventRun>& runs) {
     run_ptr_.clear(); run_n_.clear();
-    size_t n = 0;
-    for (const auto& r : runs) { run_ptr_.push_back(r.data); run_n_.push_back(r.n); n += r.n; }
-    if (esvo_ts_push_event_array(cs_->ctx(), cam_, run_ptr_.data(), run_n_.data(), (int)runs.size()) != ESVO_OK) return false;
-    pushed_ += n;
-    return true;
+    for (const auto& r : runs) { run_ptr_.push_back(r.data); run_n_.push_back(r.n); }
+    return esvo_ts_push_event_array(cs_->ctx(), cam_, run_ptr_.data(), run_n_.data(), (int)runs.size()) == ESVO_OK;
   }
-  // events pushed since construction / clearEventQueue: the `total` of the event windows read from this camera's log
-  // (esvo_events_window_dev, esvo_events_lower_bound_dev)
-  size_t eventsPushed() const { return pushed_; }
+  // events in this camera's log since construction / clearEventQueue (those a hot-pixel mask kept): the `total` of the
+  // event windows read from the log (esvo_events_window_dev, esvo_events_lower_bound_dev)
+  size_t eventsPushed() const {
+    int64_t total = 0;
+    esvo_ts_events_pushed(cs_->ctx(), cam_, &total);
+    return (size_t)total;
+  }
   // syncCallback -> createTimeSurfaceAtTime (TimeSurface.cpp:52-152,293-311); time_surface_out: H*W mono8 or nullptr
   bool createTimeSurfaceAtTime(int64_t external_sync_time_ns, uint8_t* time_surface_out) {
     return esvo_ts_build(cs_->ctx(), cam_, external_sync_time_ns, nullptr, time_surface_out) == ESVO_OK;
   }
-  void clearEventQueue() { esvo_ts_reset(cs_->ctx(), cam_); pushed_ = 0; }
+  void clearEventQueue() { esvo_ts_reset(cs_->ctx(), cam_); }
   // The reference tolerates stamps that arrive out of order (its insertion sort then re-queues events_.back(),
   // TimeSurface.cpp:410-422).  Off by default here (drivers deliver ordered packets; saves two kernels per push);
   // switch it on for sources that do not guarantee ordering -- results are then identical to the reference's.
@@ -169,7 +169,6 @@ class TimeSurface {
   std::vector<uint8_t> p_;
   std::vector<const uint8_t*> run_ptr_;
   std::vector<size_t> run_n_;
-  size_t pushed_ = 0;
 };
 }  // namespace esvo_time_surface
 

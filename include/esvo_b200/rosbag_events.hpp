@@ -235,6 +235,9 @@ class RosBagEvents {
   }
   size_t total() const { return total_; }
   size_t taken() const { return taken_; }
+  // every non-empty message's event block, in file order, whatever takeBefore has handed out (e.g. for a hot-pixel count
+  // over the whole topic, esvo_hotpix_count_event_array)
+  const std::vector<EventRun>& runs() const { return msgs_; }
   bool done() const { return k_ == msgs_.size(); }
   // stamp of the next event not handed out (undefined once done())
   int64_t nextStamp() const { return detail::wireStamp(msgs_[k_].data + pos_ * kEventWireBytes); }
