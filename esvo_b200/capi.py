@@ -600,3 +600,60 @@ class Backend:
     def launch_count(self):
         f = self.L.fn("launch_count"); f.argtypes = [C.c_void_p]; f.restype = C.c_uint64
         return int(f(self.ctx))
+
+
+# ---------------------------------------------------------------- the chunk inflater (include/esvo_b200_inflate.h)
+CODEC_BZ2, CODEC_LZ4 = 1, 2
+
+
+class Chunk(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("src_size", C.c_uint64), ("dst", C.c_void_p), ("dst_size", C.c_uint64),
+                ("codec", C.c_int32), ("status", C.c_int32)]
+
+
+class Inflater:
+    """esvo_inflater: compressed bag chunks inflated on a device; no esvo_ctx needed."""
+
+    def __init__(self, lib: Library, device: int = 0, scratch_bytes: int = 1 << 30):
+        self.lib, self.h = lib, C.c_void_p()
+        f = lib.fn("inflater_create")
+        f.argtypes = [C.c_int, C.c_size_t, C.POINTER(C.c_void_p)]
+        f.restype = C.c_int
+        rc = f(device, scratch_bytes, C.byref(self.h))
+        if rc != 0:
+            raise EsvoError(rc, "esvo_inflater_create")
+
+    def last_error(self) -> str:
+        f = self.lib.fn("inflater_last_error")
+        f.argtypes = [C.c_void_p]
+        f.restype = C.c_char_p
+        return f(self.h).decode()
+
+    def inflate(self, chunks, ok=(0,)):
+        """chunks: [(codec, src bytes, dst_size)] -> (return code, [status], [output bytes or None for a refused chunk])."""
+        srcs = [np.frombuffer(s, np.uint8) if not isinstance(s, np.ndarray) else _arr(s, np.uint8).ravel() for _, s, _ in chunks]
+        dsts = [np.empty(int(m), np.uint8) for _, _, m in chunks]
+        arr = (Chunk * max(1, len(chunks)))()
+        for k, ((codec, _, m), s, d) in enumerate(zip(chunks, srcs, dsts)):
+            arr[k] = Chunk(s.ctypes.data if s.size else None, s.size, d.ctypes.data if d.size else None, int(m), codec, 0)
+        f = self.lib.fn("inflate_chunks")
+        f.argtypes = [C.c_void_p, C.POINTER(Chunk), C.c_int]
+        f.restype = C.c_int
+        rc = f(self.h, arr, len(chunks))
+        if rc not in ok:
+            raise EsvoError(rc, "esvo_inflate_chunks", self.last_error())
+        st = [arr[k].status for k in range(len(chunks))]
+        return rc, st, [d.tobytes() if s == 0 else None for d, s in zip(dsts, st)]
+
+    def close(self):
+        if self.h:
+            f = self.lib.fn("inflater_destroy")
+            f.argtypes = [C.c_void_p]
+            f(self.h)
+            self.h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

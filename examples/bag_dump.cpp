@@ -5,8 +5,13 @@
 //                                                        per query u64 runs, u64 events; then every handed-out record
 //   bag_dump calib <bag> <topic> <out.bin>               a CameraInfo topic: esvo_calib, then esvo_compute_rectify_tables'
 //                                                        map1, map2 (f32), lut (f64 x 2), mask (u8), H*W each
-// Exit codes: 0 done, 3 the bag was refused (the reason is printed), 64 usage.
+//   A leading `--inflate-device N` opens the bag with RosBag(path, N): its bz2 / lz4 chunks are inflated on CUDA device N
+//   (include/esvo_b200_inflate.h).  Without it the bag is read on the host only and compressed chunks are refused.
+// Exit codes: 0 done, 2 compressed chunks and no CUDA device to inflate them on, 3 the bag was refused (the reason is
+// printed), 64 usage.
 #include <cstdio>
+#include <cstdlib>
+#include <memory>
 #include <fstream>
 #include <string>
 #include <vector>
@@ -16,13 +21,21 @@
 template <class T> static void wr(std::ofstream& o, const T* p, size_t n) { o.write((const char*)p, (std::streamsize)(n * sizeof(T))); }
 
 int main(int argc, char** argv) {
+  int inflate_device = -1;
+  if (argc > 2 && std::string(argv[1]) == "--inflate-device") {
+    inflate_device = std::atoi(argv[2]);
+    argv += 2; argc -= 2;
+  }
   const std::string mode = argc > 1 ? argv[1] : "";
   if (!((mode == "events" && argc == 5) || (mode == "take" && argc == 6) || (mode == "calib" && argc == 5))) {
-    std::printf("usage: bag_dump events|calib <bag> <topic> <out.bin> | bag_dump take <bag> <topic> <queries.bin> <out.bin>\n");
+    std::printf("usage: bag_dump [--inflate-device N] events|calib <bag> <topic> <out.bin> | "
+                "bag_dump [--inflate-device N] take <bag> <topic> <queries.bin> <out.bin>\n");
     return 64;
   }
   try {
-    esvo::RosBag bag(argv[2]);
+    std::unique_ptr<esvo::RosBag> owned = inflate_device < 0 ? std::make_unique<esvo::RosBag>(argv[2])
+                                                             : std::make_unique<esvo::RosBag>(argv[2], inflate_device);
+    const esvo::RosBag& bag = *owned;
     std::ofstream o(argv[argc - 1], std::ios::binary);
     if (mode == "calib") {
       const esvo_calib c = esvo::cameraInfoCalib(bag, argv[3]);
@@ -56,6 +69,9 @@ int main(int argc, char** argv) {
       all.insert(all.end(), runs.begin(), runs.end());
     }
     for (const auto& r : all) wr(o, r.data, r.n * esvo::kEventWireBytes);
+  } catch (const esvo::InflateDeviceError& e) {
+    std::printf("%s\n", e.what());
+    return 2;
   } catch (const std::exception& e) {
     std::printf("%s\n", e.what());
     return 3;

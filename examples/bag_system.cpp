@@ -1,6 +1,8 @@
 // The closed stereo-odometry loop (include/esvo_b200/esvo_system.hpp) on a recorded ROS1 bag, without ROS: the rig comes
 // from the two sensor_msgs/CameraInfo topics, the events from the two dvs_msgs/EventArray topics, and each tick's events go
 // to the device as they lie in the memory-mapped bag (esvo::RosBagEvents::takeBefore -> esvo_ts_push_event_array).
+// The bag is opened with RosBag(path, 0): bz2 and lz4 chunks (rosbag record -j / --lz4, rosbag compress) are inflated on
+// device 0 before the first tick (include/esvo_b200_inflate.h); a bag without compressed chunks creates no inflater.
 // Parameters: the hkust yamls (examples/system_common.hpp, as examples/system_loop.cpp).  Writes the result file,
 // trajectory and calls file of system_loop.cpp.
 // usage: bag_system <bag> <left events topic> <right events topic> <left camera_info topic> <right camera_info topic>
@@ -11,8 +13,8 @@
 //   --hot-pixels K: before the first tick, count each events topic over the whole bag, select the hot pixels with k = K
 //   (include/esvo_b200_hotpix.h; 5 is the usual choice) and drop their events from then on, as the offline hot-pixel tool
 //   of the reference's data preparation does; prints the number of hot pixels per camera.
-// Exit codes: 0 done, 2 no CUDA device, 3 the bag cannot be read or its hot pixels cannot be selected (the reason is
-// printed), 64 usage.
+// Exit codes: 0 done, 2 no CUDA device (also: compressed chunks and no device to inflate them on), 3 the bag cannot be read
+// (e.g. a compressed chunk is refused) or its hot pixels cannot be selected (the reason is printed), 64 usage.
 #include <chrono>
 #include <cmath>
 #include <cstdio>
@@ -58,12 +60,17 @@ int main(int argc, char** argv) {
   std::unique_ptr<esvo::RosBagEvents> ev[2];
   esvo_calib cal[2];
   try {
-    bag = std::make_unique<esvo::RosBag>(argv[1]);
+    const auto i0 = std::chrono::steady_clock::now();
+    bag = std::make_unique<esvo::RosBag>(argv[1], 0);
+    if (bag->inflatedBytes())
+      std::printf("inflated %zu bytes of compressed chunks in %.3f ms\n", bag->inflatedBytes(),
+                  std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - i0).count());
     for (int c = 0; c < 2; ++c) {
       ev[c] = std::make_unique<esvo::RosBagEvents>(*bag, argv[2 + c]);
       cal[c] = esvo::cameraInfoCalib(*bag, argv[4 + c]);
     }
-  } catch (const std::exception& e) { std::printf("%s\n", e.what()); return 3; }
+  } catch (const esvo::InflateDeviceError& e) { std::printf("%s\n", e.what()); return 2; }
+  catch (const std::exception& e) { std::printf("%s\n", e.what()); return 3; }
   if (t0 == INT64_MIN) t0 = (ev[0]->done() ? 0 : ev[0]->nextStamp()) + dt;
 
   esvo::CameraSystem::Ptr cs;

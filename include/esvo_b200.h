@@ -486,4 +486,5 @@ ESVO_API const char* esvo_version(void);
 
 #include "esvo_b200_bag.h"   /* the packed event ingest (no oracle counterpart) */
 #include "esvo_b200_hotpix.h"   /* hot pixels at the packed ingest (no oracle counterpart) */
+#include "esvo_b200_inflate.h"   /* compressed bag chunks inflated on the device (no oracle counterpart) */
 #endif /* ESVO_B200_H_ */

@@ -6,7 +6,9 @@
 // "op" naming the record type.  The records are scanned in file order:
 //   0x03 bag header            -- checked, nothing else is needed from it;
 //   0x05 chunk                 -- compression=none: its data is again a sequence of records, scanned in place; bz2 / lz4
-//                                 are refused (this library takes on no decompression dependency);
+//                                 are refused by RosBag(path); RosBag(path, inflate_device) inflates them first, on the
+//                                 device (include/esvo_b200_inflate.h: no decompression library), and scans the inflated
+//                                 bytes;
 //   0x07 connection            -- conn id -> topic and type (inside chunks and in the index section; either suffices);
 //   0x02 message data          -- conn id, receipt time, the serialised message, used where it lies in the map;
 //   0x04 index data, 0x06 chunk info -- skipped.
@@ -35,30 +37,35 @@
 
 namespace esvo {
 
+// The inflating reader found compressed chunks but could not get a CUDA device to inflate them on.
+struct InflateDeviceError : std::runtime_error {
+  using std::runtime_error::runtime_error;
+};
+
 class RosBag {
  public:
   struct Message { uint32_t conn; uint64_t time; const uint8_t* data; size_t size; };
   struct Connection { std::string topic, type; };
 
+  // Host only: a bag with a compressed chunk is refused.
   explicit RosBag(const std::string& path) {
-    const int fd = ::open(path.c_str(), O_RDONLY);
-    if (fd < 0) throw std::runtime_error("rosbag: cannot open " + path);
-    struct stat st {};
-    if (::fstat(fd, &st) != 0) { ::close(fd); throw std::runtime_error("rosbag: cannot stat " + path); }
-    size_ = (size_t)st.st_size;
-    if (size_) {
-      void* m = ::mmap(nullptr, size_, PROT_READ, MAP_PRIVATE, fd, 0);
-      ::close(fd);
-      if (m == MAP_FAILED) throw std::runtime_error("rosbag: cannot map " + path);
-      base_ = (const uint8_t*)m;
-    } else {
-      ::close(fd);
-    }
+    map(path);
     try { scan(); } catch (...) { unmap(); throw; }
+  }
+  // Inflating: the bz2 and lz4 chunks are inflated on device inflate_device (an inflater with `scratch` bytes of device
+  // memory, created only if the bag has such a chunk) in one esvo_inflate_chunks call, into host memory the RosBag owns
+  // for its lifetime; the messages of those chunks point there.  This costs host memory equal to the uncompressed chunks.
+  // A bag without compressed chunks is read as RosBag(path) reads it.
+  RosBag(const std::string& path, int inflate_device, size_t scratch = size_t(1) << 30) {
+    map(path);
+    try { inflate(inflate_device, scratch); scan(); } catch (...) { unmap(); throw; }
   }
   ~RosBag() { unmap(); }
   RosBag(const RosBag&) = delete;
   RosBag& operator=(const RosBag&) = delete;
+
+  // bytes of inflated chunk data the bag holds (0 without compressed chunks)
+  size_t inflatedBytes() const { return inflated_.size(); }
 
   const std::map<uint32_t, Connection>& connections() const { return conns_; }
   // the type of a topic ("" if the bag has no connection on it)
@@ -85,6 +92,21 @@ class RosBag {
   static uint64_t u64(const uint8_t* p) { uint64_t v; std::memcpy(&v, p, 8); return v; }
   [[noreturn]] static void truncated() { throw std::runtime_error("rosbag: truncated file"); }
 
+  void map(const std::string& path) {
+    const int fd = ::open(path.c_str(), O_RDONLY);
+    if (fd < 0) throw std::runtime_error("rosbag: cannot open " + path);
+    struct stat st {};
+    if (::fstat(fd, &st) != 0) { ::close(fd); throw std::runtime_error("rosbag: cannot stat " + path); }
+    size_ = (size_t)st.st_size;
+    if (size_) {
+      void* m = ::mmap(nullptr, size_, PROT_READ, MAP_PRIVATE, fd, 0);
+      ::close(fd);
+      if (m == MAP_FAILED) throw std::runtime_error("rosbag: cannot map " + path);
+      base_ = (const uint8_t*)m;
+    } else {
+      ::close(fd);
+    }
+  }
   void unmap() { if (base_) ::munmap((void*)base_, size_); base_ = nullptr; }
 
   static Fields fields(const uint8_t* p, size_t n) {
@@ -132,6 +154,13 @@ class RosBag {
           if (in_chunk) throw std::runtime_error("rosbag: chunk inside a chunk");
           ++chunks_;
           const std::string comp = str(field(f, "compression", 0));
+          const auto inf = inflated_at_.find(data);
+          if (inf != inflated_at_.end()) {
+            records(inflated_.data() + inf->second.first, inf->second.second, true);
+            break;
+          }
+          if (comp != "none" && inflating_)
+            throw std::runtime_error("rosbag: chunk compression '" + comp + "' is not supported (none, bz2 and lz4 are)");
           if (comp != "none")
             throw std::runtime_error("rosbag decompress: chunk compression '" + comp +
                                      "' is not supported (only uncompressed bags; `rosbag decompress` the file first)");
@@ -154,7 +183,7 @@ class RosBag {
       }
     }
   }
-  void scan() {
+  void checkMagic() const {
     static const char magic[] = "#ROSBAG V2.0\n";
     if (size_ >= 9 && std::memcmp(base_, "#ROSBAG V", 9) == 0 && (size_ < 13 || std::memcmp(base_, magic, 13) != 0)) {
       size_t e = 9;
@@ -162,13 +191,73 @@ class RosBag {
       throw std::runtime_error("rosbag: unsupported bag version V" + std::string((const char*)base_ + 9, e - 9) + " (only 2.0)");
     }
     if (size_ < 13 || std::memcmp(base_, magic, 13) != 0) throw std::runtime_error("rosbag: not a ROS bag");
+  }
+  void scan() {
+    checkMagic();
     records(base_ + 13, size_ - 13, false);
     // a file cut at a record boundary: the bag header, chunks or the index section are missing
     if (!have_header_ || chunks_ < chunk_count_ || index_pos_ > size_) truncated();
   }
 
+  // Walks the top-level records, collects the bz2 / lz4 chunks (their header's `size` is required) and inflates them all
+  // in one call.
+  void inflate(int device, size_t scratch) {
+    inflating_ = true;
+    checkMagic();
+    std::vector<esvo_chunk> cs;
+    std::vector<size_t> at;   // file offset of each chunk record
+    size_t o = 13, total = 0;
+    while (o < size_) {
+      const size_t rec = o;
+      if (size_ - o < 4) truncated();
+      const uint32_t hl = u32(base_ + o); o += 4;
+      if (hl > size_ - o) truncated();
+      const Fields f = fields(base_ + o, hl); o += hl;
+      if (size_ - o < 4) truncated();
+      const uint32_t dl = u32(base_ + o); o += 4;
+      if (dl > size_ - o) truncated();
+      const uint8_t* data = base_ + o; o += dl;
+      if (field(f, "op", 1).first[0] != 0x05) continue;
+      const std::string comp = str(field(f, "compression", 0));
+      if (comp != "bz2" && comp != "lz4") continue;
+      esvo_chunk c{};
+      c.src = data; c.src_size = dl;
+      c.dst_size = u32(field(f, "size", 4).first);
+      c.codec = comp == "bz2" ? ESVO_CODEC_BZ2 : ESVO_CODEC_LZ4;
+      cs.push_back(c); at.push_back(rec);
+      total += c.dst_size;
+    }
+    if (cs.empty()) return;
+    inflated_.resize(total);
+    size_t off = 0;
+    for (esvo_chunk& c : cs) {
+      c.dst = inflated_.data() + off;
+      inflated_at_[c.src] = {off, (size_t)c.dst_size};
+      off += c.dst_size;
+    }
+    esvo_inflater* inf = nullptr;
+    const int rc = esvo_inflater_create(device, scratch, &inf);
+    if (rc == ESVO_ERR_NO_DEVICE)
+      throw InflateDeviceError("rosbag: the bag has compressed chunks and there is no CUDA device " + std::to_string(device) +
+                               " to inflate them on (no CPU fallback)");
+    if (rc != ESVO_OK) throw InflateDeviceError("rosbag: cannot create an inflater on device " + std::to_string(device));
+    const int r = esvo_inflate_chunks(inf, cs.data(), (int)cs.size());
+    std::string why = esvo_inflater_last_error(inf);
+    esvo_inflater_destroy(inf);
+    if (r == ESVO_OK) return;
+    const size_t colon = why.find(": ");
+    if (why.compare(0, 6, "chunk ") == 0 && colon != std::string::npos) why = why.substr(colon + 2);   // the reason alone
+    for (size_t k = 0; k < cs.size(); ++k)
+      if (cs[k].status != ESVO_OK)
+        throw std::runtime_error("rosbag: compressed chunk at file offset " + std::to_string(at[k]) + " refused: " + why);
+    throw std::runtime_error("rosbag: inflating the compressed chunks failed: " + why);
+  }
+
   const uint8_t* base_ = nullptr;
   size_t size_ = 0;
+  bool inflating_ = false;
+  std::vector<uint8_t> inflated_;                                        // the inflated chunks, in file order
+  std::map<const uint8_t*, std::pair<size_t, size_t>> inflated_at_;    // chunk data in the map -> (offset, size) in inflated_
   bool have_header_ = false;
   uint64_t index_pos_ = 0;
   uint32_t chunk_count_ = 0, chunks_ = 0;
